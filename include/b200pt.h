@@ -565,6 +565,11 @@ int b200pt_bvh_info(b200pt_t* h, uint64_t* node_bytes, uint64_t* tri_bytes, uint
 int b200pt_bsdf_eval(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out);
 int b200pt_bsdf_sample(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out);
 
+/* Texture unit-test hook: n lookups against the current scene; device pointers.
+ * in: 8 floats per item (see vk_gltf_renderer_b200/tex_io.py); out: 4 floats (rgba) per item.
+ * B200PT_E_INVALID without a scene, or if a record's texture-info slot is outside the scene's. */
+int b200pt_texture_lookup(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out);
+
 #ifdef __cplusplus
 }
 #endif

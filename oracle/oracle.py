@@ -54,6 +54,7 @@ def lib():
         L.oracle_rand.argtypes = [C.c_void_p]
         L.oracle_safe_offset_ray.argtypes = [C.c_void_p] * 3
         L.oracle_sample_texture.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p]
+        L.oracle_texture_lookup.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         _lib = L
     return _lib
 
@@ -165,6 +166,14 @@ class Oracle:
     def sample_texture(self, tex, u, v, g=0.0):
         out = np.zeros(4, np.float32)
         self.L.oracle_sample_texture(self.h, tex, u, v, g, _p(out))
+        return out
+
+    def texture_lookup(self, records):
+        """getTexture / sampleLevel0 on the records of vk_gltf_renderer_b200.tex_io: rgba float32 [n, 4]"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 8)
+        out = np.empty((len(records), 4), np.float32)
+        if self.L.oracle_texture_lookup(self.h, _p(records), len(records), _p(out)):
+            raise ValueError("oracle_texture_lookup: a record has a texture-info slot outside the scene or a mode other than 0 / 1")
         return out
 
 

@@ -264,12 +264,13 @@ static float4 sampleLevel(const Texture& T, int level, float2 uv, bool linear)
 }
 
 // lambda = log2(max(|ddx * size|, |ddy * size|)); lambda <= 0 -> magnification (level 0).
-// Sampler quirk kept from the reference: the mip mode follows magFilter (gltf_scene_vk.cpp:938-942).
+// Sampler quirks kept from the reference: the mip mode follows magFilter, and magFilter goes through the same table
+// as minFilter, so 9984 / 9986 there are NEAREST too (gltf_scene_vk.cpp:922-942).
 static float4 sampleTexture(const Texture& T, float2 uv, float2 ddx, float2 ddy, bool useGrad)
 {
-  const bool magLinear = (T.magFilter != 9728);
+  const bool magLinear = !(T.magFilter == 9728 || T.magFilter == 9984 || T.magFilter == 9986);
   const bool minLinear = !(T.minFilter == 9728 || T.minFilter == 9984 || T.minFilter == 9986);
-  const bool mipLinear = (T.magFilter != 9728);
+  const bool mipLinear = magLinear;
   if(!useGrad)
     return sampleLevel(T, 0, uv, magLinear);
   const float w = (float)T.mips[0].w, h = (float)T.mips[0].h;
@@ -2579,5 +2580,26 @@ void oracle_sample_texture(void* h, int tex, float u, float v, float g, float* r
   rgba[1] = r.y;
   rgba[2] = r.z;
   rgba[3] = r.w;
+}
+// texture unit-test hook, the records of b200pt_texture_lookup (vk_gltf_renderer_b200/tex_io.py): texture-info slot, mode
+// (0 getTexture, 1 sampleLevel0 on the selected texture coordinate), tc0.xy, tc1.xy, texGrad, pad -> rgba
+int oracle_texture_lookup(void* h, const float* in, uint32_t n, float* out)
+{
+  Oracle& o = *(Oracle*)h;
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float* p = in + (size_t)i * 8;
+    if(!(p[0] >= 0.0f && p[0] < (float)o.texInfos.size() && p[0] == floorf(p[0])) || !(p[1] == 0.0f || p[1] == 1.0f))
+      return -1;
+    const b200pt_texture_info& ti = o.texInfos[(size_t)p[0]];
+    const float2               tc[2] = {f2(p[2], p[3]), f2(p[4], p[5])};
+    const float4               r = p[1] == 0.0f ? getTexture(o, ti, tc, p[6]) : sampleLevel0(o, ti, tc[ti.texCoord]);
+    float*                     q = out + (size_t)i * 4;
+    q[0] = r.x;
+    q[1] = r.y;
+    q[2] = r.z;
+    q[3] = r.w;
+  }
+  return 0;
 }
 }

@@ -113,22 +113,35 @@ def test_thin_walled_scattering_material_is_not_truncated(std_env, oracle_mod):
 
 
 def test_malformed_scene_is_rejected(box_scene, std_env):
-    """Out-of-range indices / material ids / texture slots return B200PT_E_INVALID instead of reading out of bounds."""
+    """Out-of-range indices / material ids / texture slots return B200PT_E_INVALID instead of reading out of bounds; so do
+    textures the device cannot sample like the reference: a side of 65536 or more (a 17th mip level, beyond the 16 the
+    device stores) and sampler enums getSampler does not map."""
     import copy
     from vk_gltf_renderer_b200 import synth
     from vk_gltf_renderer_b200.renderer import B200PTError, PathTracer, Resources
-    for what in ("index", "material", "slot"):
+    tex = {"tex_65536x1": (np.zeros((1, 65536, 4), np.uint8), {}), "tex_1x65536": (np.zeros((65536, 1, 4), np.uint8), {}),
+           "wrap": (np.zeros((4, 4, 4), np.uint8), dict(wrapT=33069)), "mag": (np.zeros((4, 4, 4), np.uint8), dict(magFilter=9730)),
+           "min": (np.zeros((4, 4, 4), np.uint8), dict(minFilter=9983))}
+    for what in ("index", "material", "slot") + tuple(tex):
         scn = synth.scene_from_state(copy.deepcopy(synth.scene_state(box_scene)))
         if what == "index":
             scn.render_prims[0]["indices"] = scn.render_prims[0]["indices"].copy()
             scn.render_prims[0]["indices"][0, 0] = 1 << 20
         elif what == "material":
             scn.render_nodes[0]["materialID"] = 99
-        else:
+        elif what == "slot":
             scn.materials[0].pbrBaseColorTexture = 77
+        else:
+            scn.add_texture(tex[what][0], **tex[what][1])
         pt = PathTracer(0)
-        with pytest.raises(B200PTError):
+        with pytest.raises(B200PTError, match="65536" if what.startswith("tex") else None):
             pt.onAttach(Resources(scene=scn, hdr_rgb=std_env, camera=scn.camera, size=(16, 16)))
+    # the largest texture the device does store: a side of 32768, 16 levels, the coarsest one sampled beyond the chain
+    scn = synth.scene_from_state(copy.deepcopy(synth.scene_state(box_scene)))
+    img = np.zeros((1, 32768, 4), np.uint8)
+    img[..., 3] = 255
+    scn.add_texture(img, magFilter=9728)
+    PathTracer(0).onAttach(Resources(scene=scn, hdr_rgb=std_env, camera=scn.camera, size=(16, 16)))
 
 
 def test_selection_ids_and_ndc_depth_of_frame_zero(std_env, oracle_mod):

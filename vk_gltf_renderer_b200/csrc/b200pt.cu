@@ -1723,6 +1723,32 @@ __global__ void k_bsdf_sample(const float* __restrict__ in, uint32_t n, float* _
   q[7] = (float)d.event_type;
 }
 
+// texture unit-test hook: one production lookup per record (layout in vk_gltf_renderer_b200/tex_io.py) --
+// mode 0 the shade path's getTexture, mode 1 the generic alpha test's sampleLevel0 on the selected texture coordinate
+__global__ void k_texture_lookup(DevScene S, const float* __restrict__ in, uint32_t n, float* __restrict__ out)
+{
+  stageSrgbLut(S.lutSrgb);
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if(i >= n)
+    return;
+  const float*   p = in + (size_t)i * 8;
+  const uint16_t slot = (uint16_t)p[0];
+  const float2   tc0 = f2(p[2], p[3]), tc1 = f2(p[4], p[5]);
+  float4         r;
+  if(p[1] == 0.0f)
+    r = getTexture(S, slot, tc0, tc1, p[6]);
+  else
+  {
+    const b200pt_texture_info ti = S.texInfos[slot];
+    r = sampleLevel0(S, ti, ti.texCoord ? tc1 : tc0);
+  }
+  float* q = out + (size_t)i * 4;
+  q[0] = r.x;
+  q[1] = r.y;
+  q[2] = r.z;
+  q[3] = r.w;
+}
+
 // -------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------
@@ -1757,6 +1783,7 @@ struct b200pt
   uint32_t                 ommTriangles = 0;  // non-opaque triangles of the scene that got a micromap / special state
   DevScene            S{};
   bool                haveScene = false;
+  uint32_t            numTextureInfos = 0;  // S.texInfos entries (host copy of the count, for argument checks)
   bool                hasVolume = false;
   int                 refillThreshold = kRefillThresholdDefault, postponeShift = 2;  // B200PT_REFILL / B200PT_POSTPONE env overrides (tuning)
   int                 bvhBuilder = 0;  // 0: host SAH builder (bvh.cpp), 1: device LBVH (lbvh.cuh); b200pt_set_bvh_builder / B200PT_BVH_BUILDER
@@ -2277,16 +2304,18 @@ void packTiled(const MipChain& mc, std::vector<uint32_t>& texels, uint32_t level
 void describeTexture(const b200pt_texture& src, const MipChain& mc, DevTex& dev)
 {
   const int levels = (int)std::min<size_t>(mc.level.size(), 16);
-  // sampler quirks kept from getSampler (src/gltf_scene_vk.cpp:909-947): the mip mode follows magFilter
+  // sampler quirks kept from getSampler (src/gltf_scene_vk.cpp:909-947): the mip mode follows magFilter, and magFilter goes
+  // through the same table as minFilter (9728 / 9984 / 9986 are NEAREST)
+  const bool magNearest = src.magFilter == 9728 || src.magFilter == 9984 || src.magFilter == 9986;
   dev.w0 = src.width;
   dev.h0 = src.height;
   dev.maxLevel = (float)(levels - 1);
   dev.wrapS = src.wrapS;
   dev.wrapT = src.wrapT;
   dev.srgb = src.srgb ? 1 : 0;
-  dev.magLinear = (src.magFilter != 9728) ? 1 : 0;
+  dev.magLinear = magNearest ? 0 : 1;
   dev.minLinear = (src.minFilter == 9728 || src.minFilter == 9984 || src.minFilter == 9986) ? 0 : 1;
-  dev.mipLinear = (src.magFilter != 9728) ? 1 : 0;
+  dev.mipLinear = magNearest ? 0 : 1;
 }
 
 int gridFor(const b200pt* h, int perSM) { return h->numSMs * perSM; }
@@ -2556,6 +2585,7 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
   S.nodes = dNodes;
   S.mats = dMats;
   S.texInfos = dTi;
+  h->numTextureInfos = s->numTextureInfos;
   S.lights = dLights;
   S.numLights = (int)s->numLights;
 
@@ -2623,11 +2653,29 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
   std::vector<const uchar4*> texLevel0(s->numTextures, nullptr);  // level-0 texels (device), for the alpha-triangle records
   {
     for(uint32_t i = 0; i < s->numTextures; i++)
-      if(s->textures[i].width <= 0 || s->textures[i].height <= 0 || !s->textures[i].rgba8)
+    {
+      const b200pt_texture& t = s->textures[i];
+      if(t.width <= 0 || t.height <= 0 || !t.rgba8)
       {
         h->err = "texture without pixels";
         return B200PT_E_INVALID;
       }
+      // the device keeps 16 levels (packTiled): a side of 65536 or more has a 17th, which would be sampled as level 15
+      if(t.width >= 65536 || t.height >= 65536)
+      {
+        h->err = "texture " + std::to_string(i) + " is " + std::to_string(t.width) + "x" + std::to_string(t.height) + ": a side of 65536 or more needs more than the 16 mip levels the device stores";
+        return B200PT_E_INVALID;
+      }
+      // the glTF sampler enums getSampler maps (src/gltf_scene_vk.cpp:922-945; anything else throws there)
+      auto wrapOk = [](int m) { return m == 10497 || m == 33071 || m == 33648; };
+      auto filterOk = [](int f) { return f == -1 || f == 9728 || f == 9729 || (f >= 9984 && f <= 9987); };
+      if(!wrapOk(t.wrapS) || !wrapOk(t.wrapT) || !filterOk(t.magFilter) || !filterOk(t.minFilter))
+      {
+        h->err = "texture " + std::to_string(i) + " has a sampler enum outside glTF's (wrap " + std::to_string(t.wrapS) + "/" + std::to_string(t.wrapT)
+                 + ", filter " + std::to_string(t.magFilter) + "/" + std::to_string(t.minFilter) + ")";
+        return B200PT_E_INVALID;
+      }
+    }
     std::vector<MipChain>    chains(s->numTextures);
     std::atomic<uint32_t>    nextTex{0};
     std::vector<std::thread> workers;
@@ -4631,6 +4679,35 @@ int b200pt_bsdf_sample(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_
   CK(cudaSetDevice(h->device));
   if(n)
     k_bsdf_sample<<<(n + 127) / 128, 128, 0, h->stream>>>(dev_in, n, dev_out);
+  CK(cudaGetLastError());
+  return B200PT_OK;
+}
+
+int b200pt_texture_lookup(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out)
+{
+  if(!h)
+    return B200PT_E_INVALID;
+  if(!dev_in || !dev_out || !h->haveScene)
+  {
+    h->err = "b200pt_texture_lookup: needs a scene and device buffers";
+    return B200PT_E_INVALID;
+  }
+  CK(cudaSetDevice(h->device));
+  if(!n)
+    return B200PT_OK;
+  // the records are validated on the host: a slot beyond the scene's texture infos would read past S.texInfos
+  std::vector<float> rec((size_t)n * 8);
+  CK(cudaMemcpy(rec.data(), dev_in, rec.size() * sizeof(float), cudaMemcpyDeviceToHost));
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float slot = rec[(size_t)i * 8], mode = rec[(size_t)i * 8 + 1];
+    if(!(slot >= 0.0f && slot < (float)h->numTextureInfos && slot == floorf(slot)) || !(mode == 0.0f || mode == 1.0f))
+    {
+      h->err = "b200pt_texture_lookup: record " + std::to_string(i) + " has a texture-info slot outside the scene or a mode other than 0 / 1";
+      return B200PT_E_INVALID;
+    }
+  }
+  k_texture_lookup<<<(n + 127) / 128, 128, 2048, h->stream>>>(h->S, dev_in, n, dev_out);
   CK(cudaGetLastError());
   return B200PT_OK;
 }

@@ -383,6 +383,10 @@ class PathTracer:
     def bsdf_sample(self, in_ptr, n, out_ptr):
         self._ck(self._L.b200pt_bsdf_sample(self._h, C.c_void_p(in_ptr), n, C.c_void_p(out_ptr)), "b200pt_bsdf_sample")
 
+    def texture_lookup(self, in_ptr, n, out_ptr):
+        """n texture lookups (records of tex_io, device pointers) against the attached scene: rgba, 4 floats each"""
+        self._ck(self._L.b200pt_texture_lookup(self._h, C.c_void_p(in_ptr), n, C.c_void_p(out_ptr)), "b200pt_texture_lookup")
+
 
 def render_headless(resources, frames, *, pt=None, device=0, **pt_params):
     """The reference's headless loop (src/main.cpp:133-136 + nvapp frame loop, SURVEY.md §3.1):

@@ -356,6 +356,60 @@ def synth_layers(seed=1234, layers=14, tex_size=64, blend=False, tinted=False):
     return scn
 
 
+def sampler_layers(seed=1234):
+    """synth_layers with a texture and sampler of its own on each of 14 stacked alpha layers: non-power-of-two, N x 1 and
+    1 x N images, CLAMP_TO_EDGE and MIRRORED_REPEAT (mixed per axis), NEAREST and LINEAR magnification, uv ranges far
+    outside [0, 1], one layer on TEXCOORD_1, one KHR_materials_pbrSpecularGlossiness layer (diffuse-texture alpha), one with
+    vertex-colour alpha and one BLEND layer.  Rays meet more candidates than one any-hit walk collects, so both the
+    pre-gathered alpha records and the generic in-kernel alpha test run on every sampler state."""
+    rng = np.random.default_rng(seed)
+    scn = Scene()
+    R, C, M = 10497, 33071, 33648
+    # (w, h, wrapS, wrapT, magFilter, uv scale, uv offset, variant)
+    layers = [(37, 23, R, R, 9729, (3.7, 2.1), (0.2, -0.4), None), (5, 3, C, M, 9728, (2.5, 3.5), (-0.7, -1.2), None),
+              (64, 1, M, C, 9729, (3.0, 2.0), (-1.0, -0.5), None), (23, 37, M, M, 9728, (16.0, 12.0), (-7.0, -5.0), None),
+              (16, 16, C, C, 9729, (5.0, 5.0), (-2.0, -2.0), None), (9, 17, R, M, 9728, (1.0, 1.0), (0.0, 0.0), "uv1"),
+              (7, 7, C, R, 9729, (2.2, 1.7), (-0.6, 0.3), "specgloss"), (33, 5, R, C, 9728, (1.3, 2.4), (0.1, -0.7), "color"),
+              (37, 23, M, R, 9729, (2.9, 1.9), (-1.1, 0.4), "blend"), (1, 7, R, M, 9729, (1.0, 3.3), (0.0, -1.4), None),
+              (128, 64, R, R, 9729, (1.5, 1.5), (0.0, 0.0), None), (3, 5, M, M, 9728, (40.0, 40.0), (-13.0, -17.0), None),
+              (6, 6, C, C, 9729, (3.0, 3.0), (-1.0, -1.0), None), (11, 2, M, M, 9728, (6.0, 4.0), (-2.5, -1.5), None)]
+    for l, (w, h, ws, wt, mag, sc, off, variant) in enumerate(layers):
+        rgba = rng.integers(0, 256, (h, w, 4), dtype=np.uint8)
+        tex = scn.add_texture(rgba, srgb=True, wrapS=ws, wrapT=wt, magFilter=mag, minFilter=9987 if mag == 9729 else 9984)
+        ti = scn.add_texture_info(tex, 1 if variant == "uv1" else 0)
+        if variant == "specgloss":
+            mat = scn.add_material(pbrModel=1, pbrDiffuseFactor=[0.8, 0.7, 0.6, 1], pbrSpecularFactor=[0.04, 0.04, 0.04], pbrGlossinessFactor=0.3,
+                                   alphaMode=1, alphaCutoff=0.5, doubleSided=1, pbrDiffuseTexture=ti)
+        else:
+            mat = scn.add_material(pbrBaseColorFactor=[1, 1, 1, 1], pbrRoughnessFactor=0.8, pbrMetallicFactor=0.0, alphaMode=2 if variant == "blend" else 1,
+                                   alphaCutoff=0.5 if variant != "color" else 0.3, doubleSided=1, pbrBaseColorTexture=ti)
+
+        def quad(u, v, z=-0.15 * l, l=l):
+            return _xyz((u * 2 - 1) * 1.5 + 0.03 * l, 0.1 + v * 2.0, np.full_like(u, z))
+        pos, nrm, uv, tan, idx = param_surface(quad, 3, 3)
+        uv = (uv * np.float32(sc) + np.float32(off)).astype(np.float32)
+        uv1, col = None, None
+        if variant == "uv1":
+            uv1, uv = uv * np.float32(3.1) - np.float32(1.2), uv[:, ::-1].copy()
+        if variant == "color":
+            a = _u8(rng.random(len(pos))).astype(np.uint32)
+            col = np.uint32(0x00FFFFFF) | (a << 24)
+        scn.add_node(scn.add_primitive(pos, idx, normals=nrm, uv0=uv, uv1=uv1, tangents=tan, colors=col), mat)
+
+    def ground(u, v):
+        return _xyz((u * 2 - 1) * 5, np.zeros_like(u), (1 - v * 2) * 5)
+    gp, gn, guv, gt, gi = param_surface(ground, 4, 4, (2, 2))
+    gm = scn.add_material(pbrBaseColorFactor=[0.7, 0.7, 0.7, 1], pbrRoughnessFactor=0.9, pbrMetallicFactor=0.0)
+    scn.add_node(scn.add_primitive(gp, gi, normals=gn, uv0=guv, tangents=gt), gm)
+    cam = Camera()
+    cam.eye = np.array([0.4, 1.3, 3.0], np.float32)
+    cam.center = np.array([0.0, 1.0, -1.0], np.float32)
+    cam.yfov = math.radians(50.0)
+    cam.znear, cam.zfar = 0.05, 100.0
+    scn.camera = cam
+    return scn
+
+
 def synth_helmet(seed=1234, tex_size=2048):
     """Stand-in for DamagedHelmet (BASELINE config 2; the Khronos asset is not available offline): ONE mesh of 46 080 triangles with
     ONE material that binds base colour (sRGB), metallic-roughness, normal and emissive textures of tex_size^2, floating in the
@@ -453,12 +507,14 @@ def synth_lit(seed=1234, tex_size=64):
     return scn
 
 
-def synth_material_zoo(seed=1234, tex_size=64):
+def synth_material_zoo(seed=1234, tex_size=64, samplers=False):
     """One sphere per KHR_materials_* extension, every extension WITH its textures (all 22 slots of GltfShadeMaterial that
     the path tracer reads are bound somewhere; gltf_material_eval.h.slang:168-457), plus KHR_texture_transform, TEXCOORD_1 and
     vertex colours: sheen, iridescence (+ thickness texture), anisotropy (+ direction texture), specular / specular colour,
     clearcoat (+ roughness + normal), transmission texture + thickness texture (volume), diffuse transmission (+ colour),
-    pbrSpecularGlossiness, emissive texture, BLEND alpha.  Runs the FEAT_ALL shade variant."""
+    pbrSpecularGlossiness, emissive texture, BLEND alpha.  Runs the FEAT_ALL shade variant.
+    samplers=True: the shared base-colour texture is a non-power-of-two crop with CLAMP_TO_EDGE x MIRRORED_REPEAT under a
+    rotated and scaled KHR_texture_transform, and the metallic-roughness texture is sampled NEAREST (mip mode included)."""
     rng = np.random.default_rng(seed)
     scn = Scene()
 
@@ -469,10 +525,19 @@ def synth_material_zoo(seed=1234, tex_size=64):
             a[..., 3] = alpha
         return scn.add_texture(_u8(a), srgb=srgb)
     base, mr, nm = make_texture_set(tex_size, rng, (0.8, 0.8, 0.8))
-    t_base, t_mr, t_nm = scn.add_texture(base, srgb=True), scn.add_texture(mr), scn.add_texture(nm)
     xf = (0.8, 0.3, -0.3, 0.8, 0.1, 0.2)  # KHR_texture_transform as the 2x3 matrix the loader would write
+    if samplers:
+        t_base = scn.add_texture(base[:tex_size * 3 // 5, :tex_size - 7], srgb=True, wrapS=33071, wrapT=33648)
+        t_mr, t_nm = scn.add_texture(mr, magFilter=9728, minFilter=9986), scn.add_texture(nm)
+        c, s_ = 2.5 * math.cos(0.5), 2.5 * math.sin(0.5)
+        base_xf = (c, s_ * 0.6, -s_, c * 0.6, -0.7, 0.4)   # rotation, scale (2.5, 1.5), offset
+    else:
+        t_base, t_mr, t_nm = scn.add_texture(base, srgb=True), scn.add_texture(mr), scn.add_texture(nm)
+        base_xf = None
 
     def ti(tex, texcoord=0, transform=False):
+        if tex == t_base and base_xf is not None:
+            return scn.add_texture_info(tex, texcoord, base_xf)
         return scn.add_texture_info(tex, texcoord, xf if transform else (1, 0, 0, 1, 0, 0))
     mats = [
         dict(pbrBaseColorFactor=[0.35, 0.1, 0.4, 1], pbrRoughnessFactor=0.8, pbrMetallicFactor=0.0, sheenColorFactor=[0.9, 0.8, 1.0], sheenRoughnessFactor=0.6,
