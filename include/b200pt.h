@@ -472,10 +472,48 @@ int b200pt_get_selection_device(b200pt_t* h, uint32_t** dev_object_ids, float** 
  * camera space by mul(float3x3(viewMatrix), N), normalised and compressed to 32 bits (nvshaders' compressUnitVec: octahedral,
  * 2 x 16 bits; restated, external); (0, 0, 1) where the primary ray missed.  Written by every frame whose push constants carry
  * B200PT_PT_USE_OPTIX_DENOISER, which requires b200pt_set_guide_outputs(h, 1) (the path pools grow by 32 bytes per slot; calling it
- * re-allocates them like b200pt_resize).  The DLSS variant (its extra guides, frame jitter, motion vectors) is not built. */
+ * re-allocates them like b200pt_resize). */
 int b200pt_set_guide_outputs(b200pt_t* h, int enable);
 int b200pt_read_guide(b200pt_t* h, float* host_albedo_normal, size_t num_floats);
 int b200pt_get_guide_device(b200pt_t* h, float** dev_albedo_normal, size_t* num_floats);
+
+/* The DLSS variant (reference PathtracerFlags::ePtUseDlss, shaders/gltf_pathtrace.slang:564-651): the six guide images the
+ * reference's path tracer hands to DLSS Ray Reconstruction (OutputImage::eDlss*, formats of src/dlss.cpp:61-66).  Each plane
+ * holds tile_rows x width pixels in its format, so it can be copied into a VkImage of that format:
+ *   albedo            RGBA8 UNORM   first-hit base colour (binary16-rounded), alpha 1 where the sample stayed solid
+ *   spec_albedo       RGBA16F       EnvBRDFApprox2 of the first hit's dielectric f0 x specular colour, alpha 1
+ *   normal_roughness  RGBA16F       world-space shading normal, roughness
+ *   motion            RG16F         pixel-space motion vector (camera + instance motion; sky: camera rotation only)
+ *   depth             R16F          NDC depth of the first hit (1 = miss)
+ *   spec_hit_dist     R16F          distance to the surface behind a glossy reflection of the first hit (65504 = sky, 0 = none)
+ * Pixels without a hit read 0 except depth (1) and spec_albedo's alpha (1).  A frame whose push constants carry B200PT_PT_USE_DLSS
+ * must have numSamples == 1; its sub-pixel position is 0.5 + frame_info.jitter (no Gaussian jitter is drawn), it REPLACES the
+ * accumulation image, never joins a frame batch, and writes the six planes for the newest frame.  It requires
+ * b200pt_set_dlss_guides(h, 1), which re-allocates the path pools like b200pt_resize: each slot carries 24 more bytes (previous-
+ * frame first-hit position, specular albedo + hit distance as binary16) plus the 32 bytes of the guide records if
+ * b200pt_set_guide_outputs is off, and the tile 28 bytes per pixel for the planes.  Instance motion: the first
+ * b200pt_update_transforms / b200pt_update_node_matrices after a rendered frame keeps the render nodes' objectToWorld of that
+ * frame, and the next frame reprojects its first hits through it; a frame with no update before it sees camera motion only.
+ * b200pt_read_dlss_guides copies the planes whose host pointer is not NULL (each *_bytes must hold its plane);
+ * b200pt_get_dlss_guides_device returns the device planes and their sizes. */
+typedef struct b200pt_dlss_guides
+{
+  void*  albedo;
+  size_t albedo_bytes;
+  void*  spec_albedo;
+  size_t spec_albedo_bytes;
+  void*  normal_roughness;
+  size_t normal_roughness_bytes;
+  void*  motion;
+  size_t motion_bytes;
+  void*  depth;
+  size_t depth_bytes;
+  void*  spec_hit_dist;
+  size_t spec_hit_dist_bytes;
+} b200pt_dlss_guides;
+int b200pt_set_dlss_guides(b200pt_t* h, int enable);
+int b200pt_read_dlss_guides(b200pt_t* h, const b200pt_dlss_guides* out);
+int b200pt_get_dlss_guides_device(b200pt_t* h, b200pt_dlss_guides* out);
 
 /* Tone mapping + 8-bit encode of the accumulation image: what GltfRenderer::tonemap does to gBuffers[eImgRendered] before
  * saveHeadlessOutputImage writes gBuffers[eImgTonemapped] (src/renderer.cpp:992-1054, 557-573).  The compute shader is

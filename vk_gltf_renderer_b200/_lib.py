@@ -20,6 +20,7 @@ EXPORTS = [
     "b200pt_trace_shadow", "b200pt_bvh_info", "b200pt_bsdf_eval", "b200pt_bsdf_sample", "b200pt_texture_lookup",
     "b200pt_read_selection", "b200pt_get_selection_device", "b200pt_set_frame_batch", "b200pt_flush", "b200pt_update_transforms", "b200pt_set_bvh_builder", "b200pt_bvh_build_ms",
     "b200pt_set_opacity_micromaps", "b200pt_set_animation", "b200pt_animate", "b200pt_set_node_hierarchy", "b200pt_update_node_matrices", "b200pt_tonemap", "b200pt_tonemap_image", "b200pt_get_tonemapped_device", "b200pt_set_guide_outputs", "b200pt_read_guide", "b200pt_get_guide_device",
+    "b200pt_set_dlss_guides", "b200pt_read_dlss_guides", "b200pt_get_dlss_guides_device",
 ]
 
 
@@ -91,6 +92,9 @@ def lib(count_traversal=False):
     L.b200pt_set_guide_outputs.argtypes = [vp, i32]
     L.b200pt_read_guide.argtypes = [vp, vp, C.c_size_t]
     L.b200pt_get_guide_device.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t)]
+    L.b200pt_set_dlss_guides.argtypes = [vp, i32]
+    L.b200pt_read_dlss_guides.argtypes = [vp, C.POINTER(abi.DlssGuides)]
+    L.b200pt_get_dlss_guides_device.argtypes = [vp, C.POINTER(abi.DlssGuides)]
     L.b200pt_get_selection_device.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
     for name in EXPORTS:
         getattr(L, name)  # raises AttributeError if a declared symbol is not exported

@@ -133,6 +133,13 @@ class Tonemapper(C.Structure):
                 ("contrast", C.c_float), ("saturation", C.c_float), ("vignette", C.c_float), ("autoExposure", C.c_int32)]
 
 
+class DlssGuides(C.Structure):
+    """b200pt_dlss_guides: the six DLSS guide planes (host or device pointers) and their sizes in bytes"""
+    _fields_ = [("albedo", C.c_void_p), ("albedo_bytes", C.c_size_t), ("spec_albedo", C.c_void_p), ("spec_albedo_bytes", C.c_size_t),
+                ("normal_roughness", C.c_void_p), ("normal_roughness_bytes", C.c_size_t), ("motion", C.c_void_p), ("motion_bytes", C.c_size_t),
+                ("depth", C.c_void_p), ("depth_bytes", C.c_size_t), ("spec_hit_dist", C.c_void_p), ("spec_hit_dist_bytes", C.c_size_t)]
+
+
 class RenderNodeMapping(C.Structure):
     """b200pt_render_node_mapping == RenderNodeGpuMapping (shaders/world_matrix_io.h.slang:41-47)"""
     _fields_ = [("nodeID", C.c_int32), ("pad0", C.c_int32), ("materialID", C.c_int32), ("renderPrimID", C.c_int32)]

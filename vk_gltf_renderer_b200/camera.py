@@ -101,6 +101,28 @@ def make_frame_info(cam, width, height, *, use_hdr=True, env_rotation=0.0, env_i
     return fi
 
 
+def halton(index):
+    """shaderio::halton (shaders/dlss_util.h), float32 as the host evaluates it: both bases advance in one loop that stops when
+    EITHER remainder reaches 0, so the base-2 digits beyond the base-3 length are not added."""
+    f = np.float32
+    sx = sy = f(index)
+    ax, ay, az, aw = f(1.0), f(1.0), f(0.0), f(0.0)
+    while sx > 0.0 and sy > 0.0:
+        ax = f(ax / f(2.0))
+        ay = f(ay / f(3.0))
+        az = f(az + f(ax * np.fmod(sx, f(2.0))))
+        aw = f(aw + f(ay * np.fmod(sy, f(3.0))))
+        sx = np.floor(f(sx / f(2.0)))
+        sy = np.floor(f(sy / f(3.0)))
+    return az, aw
+
+
+def dlss_jitter(frame_index):
+    """shaderio::dlssJitter: the Halton point of the DLSS frame index, centred on (0, 0) (Dlss::beginFrame, src/dlss.cpp:401-414)"""
+    hx, hy = halton(int(frame_index))
+    return np.float32(hx - np.float32(0.5)), np.float32(hy - np.float32(0.5))
+
+
 def make_push_constant(cam, height, *, frame_count, total_samples, num_samples=1, max_depth=5,
                        firefly_clamp=10.0, tex_grad_scale=1.0, aperture=0.0, focal_distance=None):
     """PathtracePushConstant as filled by setupPushConstant (renderer_pathtracer.cpp:1496-1574):

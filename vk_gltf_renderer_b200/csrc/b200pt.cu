@@ -11,6 +11,8 @@
 //   accumulation                                   gltf_pathtrace.slang:582-630          -> k_accumulate
 //   shadow catcher (handleShadowCatcher)           pathtrace_functions.h.slang:499-554   -> k_shade (light sample) + shadow kernels + finishPost
 //   eOptixAlbedoNormal guide image                 gltf_pathtrace.slang:240-263,653-670  -> capture in k_shade, k_guide
+//   DLSS variant: jitter, guides, motion vectors   gltf_pathtrace.slang:135-143,216-263,370-377,564-651 -> k_raygen, k_shade, k_dlss_guides
+//   snapshot_prev_transforms.comp                  src/renderer.cpp:630-655                               -> k_snapshot_prev_transforms
 // Next to the frame path (SURVEY.md section 8 f):
 //   morph.comp / skinning.comp                     shaders/*.comp.slang                  -> k_morph, k_skin, k_regather_shade (animate.cuh)
 //   world_matrix_propagate / update_render_instances                                     -> k_propagate_level, k_update_render_nodes
@@ -34,6 +36,7 @@
 
 #include "bvh.h"
 #include "animate.cuh"
+#include "dlss_guides.cuh"
 #include "lbvh.cuh"
 #include "shade.cuh"
 #include "tonemap.cuh"
@@ -50,6 +53,9 @@ static_assert(sizeof(b200pt_push_constant) == 48, "PathtracePushConstant layout"
 namespace {
 
 constexpr int kMaxIters = 4096;  // per-frame iteration counter slots
+// the six DLSS guide planes of one pixel: albedo RGBA8 (4 B), specular albedo RGBA16F (8), normal / roughness RGBA16F (8),
+// motion RG16F (4), depth R16F (2), specular hit distance R16F (2)
+constexpr size_t kDlssBytesPerPixel = 28;
 // Any-hit continuation rounds per bounce: a ray whose kCand candidates were all rejected goes through another k_trace / k_shadow round
 // that resumes behind the last one; after kContRoundsMax rounds whatever is still undecided finishes inside the last k_alpha.  Counter
 // arrays per lane: 5 (trace / post queues and cursors, shadow queue) + per ray kind (rounds + 1) any-hit counters, rounds continuation
@@ -162,12 +168,25 @@ __global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_consta
     const uint32_t x = px % (uint32_t)F.width;
     const uint32_t y = pixelRow(F, px);
     uint32_t       seed = xxhash32(x, y, (uint32_t)F.pc.frameCount + frameOf(F, i));
-    const float    u1 = rnd(seed), u2 = rnd(seed);
+    uint32_t       drawn = seed;
+    const float    u1 = rnd(drawn), u2 = rnd(drawn);
     // sampleGaussian (pathtrace_functions.h.slang:784-789), sigma = 0.4246609 px
-    const float  rr = sqrtf(-2.0f * logf(fmaxf(1e-38f, u1)));
-    const float  theta = 2.0f * kPi * u2;
-    const float2 jitter = f2(0.5f + (rr * cosf(theta)) * 0.4246609f, 0.5f + (rr * sinf(theta)) * 0.4246609f);
+    const float    rr = sqrtf(-2.0f * logf(fmaxf(1e-38f, u1)));
+    const float    theta = 2.0f * kPi * u2;
+    float2         jitter = f2(0.5f + (rr * cosf(theta)) * 0.4246609f, 0.5f + (rr * sinf(theta)) * 0.4246609f);
+    // the DLSS jitter moves the whole frame and the Gaussian's two rand() are not drawn (gltf_pathtrace.slang:568-572)
+    if(F.pc.flags & B200PT_PT_USE_DLSS)
+      jitter = f2(0.5f + F.fi.jitter[0], 0.5f + F.fi.jitter[1]);
+    else
+      seed = drawn;
     P.pixSum[i] = f4(0.f, 0.f, 0.f, 0.f);
+    if(isDlssFrame(P, F))
+    {
+      // a DLSS frame has one sample, started here: the first-hit scratch of every frame and the DLSS GuideScratch defaults
+      P.firstHit[i] = f4(1e34f, 1e34f, 1e34f, 1.0f);
+      P.prevHit[i] = f4(1e34f, 1e34f, 1e34f, 1.0f);  // firstHitPosPrev sentinel
+      P.dlssSpec[i] = make_uint2(0u, 0u);            // specularAlbedo 0, specularHitDist 0
+    }
     startSample(P, F, i, seed, jitter, 0u);
     qTrace[i] = i;
   }
@@ -655,13 +674,23 @@ __global__ void __launch_bounds__(SHADE_BLOCK, SHADE_MIN_BLOCKS * 128 / SHADE_BL
       if(depth == 0)
       {
         flags &= ~PF_SOLID;  // tryPrimaryMissBackplate: pt.solid = false
-        if(isFirstFrame(F, i))
+        const bool dlss = isDlssFrame(P, F);
+        if(isFirstFrame(F, i) || dlss)
           P.firstHit[i] = f4(dir, 0.0f);  // pt.firstHitPos = ray.Direction (pathtrace_functions.h.slang:950)
+        if(dlss)
+          P.prevHit[i] = f4(dir, 0.0f);  // pt.firstHitPosPrev = ray.Direction (:952-955)
         if(F.fi.flags & B200PT_SCENE_USE_SOLID_BACKGROUND)
         {
           finalizeSample(P, F, i, f3(F.fi.backgroundColor[0], F.fi.backgroundColor[1], F.fi.backgroundColor[2]), false, seed, sampleIdx, qNext, cntNext, stats);
           return false;
         }
+      }
+      if(flags & PF_SPEC_CAPTURE)
+      {
+        // a glossy reflection of the first hit went to the sky: fp16 max (gltf_pathtrace.slang:135-143)
+        uint2* const sp = &P.dlssSpec[i];
+        sp->y = (sp->y & 0xffffu) | ((uint32_t)dlssHalfBits(65504.0f) << 16);
+        flags &= ~PF_SPEC_CAPTURE;
       }
       const float3 edir = rotateAxis(dir, f3(0, 1, 0), -F.fi.envRotation);
       const float4 env = sampleEnvTex(S, getSphericalUv(edir));
@@ -730,22 +759,51 @@ __global__ void __launch_bounds__(SHADE_BLOCK, SHADE_MIN_BLOCKS * 128 / SHADE_BL
       unlit = gmat.unlit;
     }
 
+    if(flags & PF_SPEC_CAPTURE)
+    {
+      // the first surface behind a glossy reflection of the first hit (:216-223); the shadow catcher returned above, so its plane
+      // leaves the capture armed
+      uint2* const sp = &P.dlssSpec[i];
+      sp->y = (sp->y & 0xffffu) | ((uint32_t)dlssHalfBits(hitT) << 16);
+      flags &= ~PF_SPEC_CAPTURE;
+    }
+
     // firefly control: never get sharper than the roughest bounce so far (:267-268)
     misc.x = fmaxf(pbrMat.roughness.x, misc.x);
     misc.y = fmaxf(pbrMat.roughness.y, misc.y);
     pbrMat.roughness = f2(misc.x, misc.y);
 
-    // first-hit capture for the NDC depth output of frame 0 (gltf_pathtrace.slang:228-232)
-    if(depth == 0 && isFirstFrame(F, i))
+    // first-hit capture for the NDC depth output of frame 0 and, on DLSS frames, of every frame (gltf_pathtrace.slang:228-232)
+    const bool dlss = isDlssFrame(P, F);
+    if(depth == 0 && (isFirstFrame(F, i) || dlss))
       P.firstHit[i] = f4(hit.pos, 1.0f);
-    // denoiser guides of the first hit (gltf_pathtrace.slang:240-263, the USE_GUIDE_SHADER part without the DLSS-only specular guides):
-    // base colour and shading normal / roughness, stored as float16_t by the reference.  (maxRoughness is still 0 at depth 0, so the
-    // clamp above left pbrMat.roughness as evaluateMaterial returned it.)
-    if(depth == 0 && P.guideA && (F.pc.flags & B200PT_PT_USE_OPTIX_DENOISER))
+    // denoiser guides of the first hit (gltf_pathtrace.slang:240-263): base colour and shading normal / roughness, stored as
+    // float16_t by the reference.  (maxRoughness is still 0 at depth 0, so the clamp above left pbrMat.roughness as evaluateMaterial
+    // returned it.)
+    if(depth == 0 && P.guideA && (F.pc.flags & (B200PT_PT_USE_OPTIX_DENOISER | B200PT_PT_USE_DLSS)))
     {
       auto h16 = [](float x) { return __half2float(__float2half_rn(x)); };
       P.guideA[i] = f4(h16(pbrMat.baseColor.x), h16(pbrMat.baseColor.y), h16(pbrMat.baseColor.z), h16(pbrMat.roughness.x));
       P.guideN[i] = f4(h16(pbrMat.N.x), h16(pbrMat.N.y), h16(pbrMat.N.z), 1.0f);
+    }
+    if(depth == 0 && dlss)
+    {
+      // instance motion: the same surface point under the previous frame's objectToWorld (:235-241); the plane does not move
+      float3 prev = hit.pos;
+      if(!onPlane && F.prevObjectToWorld)
+      {
+        const uint32_t rnode = meta.x & 0x0fffffffu;
+        const float4   objPos = mul_vM(f4(hit.pos, 1.0f), *reinterpret_cast<const Mat4*>(nodeP->worldToObject));
+        prev = xyz(mul_vM(f4(xyz(objPos), 1.0f), *reinterpret_cast<const Mat4*>(F.prevObjectToWorld + 16u * rnode)));
+      }
+      P.prevHit[i] = f4(prev, 1.0f);
+      // specular albedo (:246-255): dielectric f0 from the ior pair (pow(x, 2) as the correctly rounded x * x), times the specular
+      // colour, clamped to 1.  The hit distance half stays 0: a capture is armed only by a depth-0 BSDF sample, after which depth > 0.
+      const float  r = (pbrMat.ior2 - pbrMat.ior1) / (pbrMat.ior2 + pbrMat.ior1);
+      const float  f0 = r * r;
+      const float3 sc = f3(fminf(f0 * pbrMat.specularColor.x, 1.0f), fminf(f0 * pbrMat.specularColor.y, 1.0f), fminf(f0 * pbrMat.specularColor.z, 1.0f));
+      const float3 sa = dlssEnvBRDFApprox2(sc, pbrMat.roughness.x, dot(pbrMat.N, dir));
+      P.dlssSpec[i] = make_uint2((uint32_t)dlssHalfBits(sa.x) | ((uint32_t)dlssHalfBits(sa.y) << 16), (uint32_t)dlssHalfBits(sa.z));
     }
 
     radiance += pbrMat.emissive * throughput;
@@ -888,6 +946,9 @@ __global__ void __launch_bounds__(SHADE_BLOCK, SHADE_MIN_BLOCKS * 128 / SHADE_BL
       throughput *= sd.bsdf_over_pdf;
       dir = sd.k2;
       lastSamplePdf = sd.pdf;
+      // DLSS: a glossy or mirror reflection of the first hit arms the specular hit-distance capture (:370-377)
+      if(depth == 0 && (sd.event_type == BSDF_EVENT_GLOSSY_REFLECTION || sd.event_type == (BSDF_EVENT_IMPULSE | BSDF_EVENT_REFLECTION)) && isDlssFrame(P, F))
+        flags |= PF_SPEC_CAPTURE;
       if(sd.event_type != BSDF_EVENT_ABSORB)
       {
         const float3 offsetDir = dot(dir, hit.geonrm) > 0 ? hit.geonrm : -hit.geonrm;
@@ -1318,7 +1379,8 @@ __global__ void __launch_bounds__(256) k_resolve(PathState P, DevScene S, const 
 }
 
 // processPixel tail: mean over the frame's samples + running mean over frames (gltf_pathtrace.slang:596,619-630); on the
-// first frame also the NDC depth of the last sample's first hit (:600-616; Vulkan [0,1] range, 1 = far / miss)
+// first frame also the NDC depth of the last sample's first hit (:600-616; Vulkan [0,1] range, 1 = far / miss).  A DLSS frame
+// replaces the image like a first frame (:619-622).
 __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_constant__ FrameParams F, float4* __restrict__ accum, float* __restrict__ ndcDepth)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
@@ -1329,10 +1391,10 @@ __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_co
     for(int b = 0; b < F.batch; b++)
     {
       const float4 c = P.pixSum[i + (uint32_t)b * F.pixels] / (float)F.pc.numSamples;
-      if(b == 0 && (F.pc.flags & B200PT_PT_FIRST_FRAME))
+      if(b == 0 && (F.pc.flags & (B200PT_PT_FIRST_FRAME | B200PT_PT_USE_DLSS)))
       {
         img = c;
-        if(ndcDepth)
+        if(ndcDepth && (F.pc.flags & B200PT_PT_FIRST_FRAME))
         {
           const float4 fh = P.firstHit[i];
           float        d = 1.0f;
@@ -1396,6 +1458,52 @@ __global__ void __launch_bounds__(256) k_guide(PathState P, const __grid_constan
     }
     guide[i] = f4(a.x, a.y, a.z, __uint_as_float(compressUnitVec(camN)));
   }
+}
+
+// The six DLSS guide images of processPixel (gltf_pathtrace.slang:628-651) for the newest frame, each plane in its format
+// (src/dlss.cpp:61-66): albedo RGBA8, specular albedo RGBA16F, normal / roughness RGBA16F, motion RG16F, depth R16F, specular hit
+// distance R16F.
+struct DlssPlanes
+{
+  uint32_t* albedo;
+  uint2*    specAlbedo;
+  uint2*    normalRough;
+  uint32_t* motion;
+  uint16_t* depth;
+  uint16_t* specHitDist;
+};
+
+__global__ void __launch_bounds__(256) k_dlss_guides(PathState P, const __grid_constant__ FrameParams F, DlssPlanes out)
+{
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels; i += stride)
+  {
+    const uint32_t slot = i + (uint32_t)(F.batch - 1) * F.pixels;
+    const float4   a = P.guideA[slot], n = P.guideN[slot];
+    const bool     solid = P.pixSum[slot].w > 0.0f;  // sampleResult.radiance.w > 0 (the firefly clamp scales it by a positive factor)
+    const DlssGuidePixel g = dlssPackGuides(xyz(a), f4(n.x, n.y, n.z, a.w), P.dlssSpec[slot], xyz(P.firstHit[slot]), xyz(P.prevHit[slot]), solid,
+                                            F.fi.viewProjMatrix, F.fi.prevMVP, f2(F.fi.imageSize[0], F.fi.imageSize[1]));
+    out.albedo[i] = g.albedo;
+    out.specAlbedo[i] = make_uint2((uint32_t)g.specAlbedo[0] | ((uint32_t)g.specAlbedo[1] << 16), (uint32_t)g.specAlbedo[2] | ((uint32_t)g.specAlbedo[3] << 16));
+    out.normalRough[i] = make_uint2((uint32_t)g.normalRough[0] | ((uint32_t)g.normalRough[1] << 16), (uint32_t)g.normalRough[2] | ((uint32_t)g.normalRough[3] << 16));
+    out.motion[i] = (uint32_t)g.motion[0] | ((uint32_t)g.motion[1] << 16);
+    out.depth[i] = g.depth;
+    out.specHitDist[i] = g.specHitDist;
+  }
+}
+
+// snapshot_prev_transforms.comp.slang: the render nodes' objectToWorld before a transform update overwrites them
+// (world_matrix_io.h.slang:65-75), one thread per render node
+__global__ void __launch_bounds__(256) k_snapshot_prev_transforms(const b200pt_render_node* __restrict__ nodes, float* __restrict__ prev, uint32_t n)
+{
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if(i >= n)
+    return;
+  // render nodes are 136 bytes apart, so their matrices are only 8-byte aligned: no 16-byte loads
+  const float* src = nodes[i].objectToWorld;
+  float*       dst = prev + 16u * i;
+  for(int k = 0; k < 16; k++)
+    dst[k] = src[k];
 }
 
 // traceSelectionRay (pathtrace_functions.h.slang:813-820) for every pixel of the first frame: the pixel-centre ray
@@ -1853,6 +1961,14 @@ struct b200pt
   float4*            dAccum = nullptr;
   bool               guides = false;      // b200pt_set_guide_outputs: the path pools carry guideA / guideN, dGuide is the eOptixAlbedoNormal image
   float4*            dGuide = nullptr;
+  // b200pt_set_dlss_guides: the path pools carry guideA / guideN + prevHit / dlssSpec, dDlss holds the six guide planes (28 B per pixel)
+  bool               dlss = false;
+  uint8_t*           dDlss = nullptr;
+  // previous-frame objectToWorld of every render node (k_snapshot_prev_transforms): taken by the first transform update after a
+  // rendered frame, read by the next frame only
+  float*             dPrevO2W = nullptr;
+  bool               prevO2WValid = false;
+  bool               renderedSinceUpdate = false;
   uchar4*            dTonemapped = nullptr;  // gBuffers[eImgTonemapped] of this tile (b200pt_tonemap), in poolAllocs
   uint32_t*          dTmHist = nullptr;      // 256-bin log2-luminance histogram + the exposure factor behind it (allocated with the handle)
   uint32_t*          dSelect = nullptr;  // frame-0 outputs (gltf_pathtrace.slang:610-616): object id per pixel ...
@@ -1983,7 +2099,7 @@ int allocPathState(b200pt* h, std::vector<void*>& owner, size_t n, PathState& P)
   }
   owner.push_back(d);
   P.candInfo = reinterpret_cast<uint2*>(d);
-  if(h->guides)
+  if(h->guides || h->dlss)
     for(float4** a : {&P.guideA, &P.guideN})
     {
       void* g = nullptr;
@@ -1996,6 +2112,23 @@ int allocPathState(b200pt* h, std::vector<void*>& owner, size_t n, PathState& P)
       owner.push_back(g);
       *a = reinterpret_cast<float4*>(g);
     }
+  if(h->dlss)
+  {
+    const size_t bytes[2] = {16, sizeof(uint2)};
+    void*        g[2] = {nullptr, nullptr};
+    for(int k = 0; k < 2; k++)
+    {
+      if(cudaMalloc(&g[k], std::max<size_t>(n, 1) * bytes[k]) != cudaSuccess)
+      {
+        cudaGetLastError();
+        h->err = "path pool: out of device memory";
+        return B200PT_E_NOMEM;
+      }
+      owner.push_back(g[k]);
+    }
+    P.prevHit = reinterpret_cast<float4*>(g[0]);
+    P.dlssSpec = reinterpret_cast<uint2*>(g[1]);
+  }
   return B200PT_OK;
 }
 
@@ -2151,6 +2284,10 @@ void freeHierarchy(b200pt* h)
 
 void freeScene(b200pt* h)
 {
+  cudaFree(h->dPrevO2W);
+  h->dPrevO2W = nullptr;
+  h->prevO2WValid = false;
+  h->renderedSinceUpdate = false;
   freeAnimation(h);
   freeHierarchy(h);
   for(void* p : h->sceneAllocs)
@@ -2183,6 +2320,7 @@ void freePool(b200pt* h)
   h->dNdcDepth = nullptr;
   h->dTonemapped = nullptr;
   h->dGuide = nullptr;
+  h->dDlss = nullptr;
   h->numPaths = 0;
   for(int l = 0; l < b200pt::kMaxLanes; l++)
   {
@@ -3376,6 +3514,23 @@ static int refitTrees(b200pt_t* h)
   return B200PT_OK;
 }
 
+// the reference snapshots objectToWorld at the start of a frame whose transforms change (src/renderer.cpp:630-655): here the first
+// transform update after a rendered frame copies the render nodes' current objectToWorld before it overwrites them, and the next
+// frame reads the copy.  Runs on the handle's stream after syncAll, so no frame in flight still reads the previous copy.
+static int snapshotPrevTransforms(b200pt_t* h)
+{
+  if(!h->renderedSinceUpdate || h->numSceneNodes == 0)
+    return B200PT_OK;
+  if(!h->dPrevO2W)
+    CK(cudaMalloc((void**)&h->dPrevO2W, (size_t)h->numSceneNodes * 16 * sizeof(float)));
+  k_snapshot_prev_transforms<<<(h->numSceneNodes + 255) / 256, 256, 0, h->stream>>>(h->dNodesW, h->dPrevO2W, h->numSceneNodes);
+  h->kernelLaunches++;
+  CK(cudaGetLastError());
+  h->prevO2WValid = true;
+  h->renderedSinceUpdate = false;
+  return B200PT_OK;
+}
+
 int b200pt_update_transforms(b200pt_t* h, const b200pt_render_node* nodes, uint32_t num_nodes)
 {
   if(!h || !h->haveScene || !nodes || num_nodes != h->numSceneNodes)
@@ -3392,6 +3547,8 @@ int b200pt_update_transforms(b200pt_t* h, const b200pt_render_node* nodes, uint3
   }
   syncAll(h);
   cudaStream_t st = h->stream;
+  if(const int rc = snapshotPrevTransforms(h))
+    return rc;
   CK(cudaMemcpyAsync(h->dNodesW, nodes, (size_t)num_nodes * sizeof(b200pt_render_node), cudaMemcpyHostToDevice, st));
   return refitTrees(h);
 }
@@ -3481,6 +3638,8 @@ int b200pt_update_node_matrices(b200pt_t* h, const float* local_matrices)
   }
   syncAll(h);
   cudaStream_t st = h->stream;
+  if(const int rc = snapshotPrevTransforms(h))
+    return rc;
   CK(cudaMemcpyAsync(h->dLocalMats, local_matrices, (size_t)h->numGraphNodes * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
   for(size_t l = 0; l + 1 < h->levelOffsets.size(); l++)
   {
@@ -3867,6 +4026,19 @@ int b200pt_resize(b200pt_t* h, int width, int height, int tile_y0, int tile_rows
     if(cudaMemsetAsync(h->dGuide, 0, n * 16, h->stream) != cudaSuccess)
       return fail(B200PT_E_CUDA);
   }
+  if(h->dlss)
+  {
+    if(cudaMalloc((void**)&h->dDlss, n * kDlssBytesPerPixel + 6 * 256) != cudaSuccess)
+    {
+      cudaGetLastError();
+      h->dDlss = nullptr;
+      h->err = "DLSS guide images: out of device memory";
+      return fail(B200PT_E_NOMEM);
+    }
+    h->poolAllocs.push_back(h->dDlss);
+    if(cudaMemsetAsync(h->dDlss, 0, n * kDlssBytesPerPixel + 6 * 256, h->stream) != cudaSuccess)
+      return fail(B200PT_E_CUDA);
+  }
   if(cudaMalloc((void**)&h->dTonemapped, n * 4) != cudaSuccess)
   {
     cudaGetLastError();
@@ -4160,6 +4332,96 @@ int b200pt_get_guide_device(b200pt_t* h, float** dev_albedo_normal, size_t* num_
   return B200PT_OK;
 }
 
+int b200pt_set_dlss_guides(b200pt_t* h, int enable)
+{
+  if(!h)
+    return B200PT_E_INVALID;
+  CK(cudaSetDevice(h->device));
+  {
+    const int frc = flushPending(h);
+    if(frc)
+      return frc;
+  }
+  if((enable != 0) == h->dlss)
+    return B200PT_OK;
+  h->dlss = enable != 0;
+  if(h->numPaths == 0)
+    return B200PT_OK;
+  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
+  int           rc;
+  if(h->bandWorld > 1)
+    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
+  else
+    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
+  if(rc == B200PT_OK && user)
+    h->dAccum = user;
+  return rc;
+}
+
+// the six planes inside dDlss, in the order of b200pt_dlss_guides; each starts on a 256-byte boundary (dlssAllocBytes)
+static void dlssPlanes(const b200pt_t* h, void* ptr[6], size_t bytes[6])
+{
+  const size_t n = h->numPaths;
+  const size_t per[6] = {4, 8, 8, 4, 2, 2};
+  size_t       off = 0;
+  for(int k = 0; k < 6; k++)
+  {
+    ptr[k] = h->dDlss + off;
+    bytes[k] = n * per[k];
+    off += (bytes[k] + 255) & ~(size_t)255;
+  }
+}
+
+int b200pt_read_dlss_guides(b200pt_t* h, const b200pt_dlss_guides* out)
+{
+  if(!h || h->numPaths == 0 || !h->dDlss || !out)
+    return B200PT_E_INVALID;
+  void*        dev[6];
+  size_t       need[6];
+  dlssPlanes(h, dev, need);
+  void* const  host[6] = {out->albedo, out->spec_albedo, out->normal_roughness, out->motion, out->depth, out->spec_hit_dist};
+  const size_t have[6] = {out->albedo_bytes, out->spec_albedo_bytes, out->normal_roughness_bytes, out->motion_bytes, out->depth_bytes, out->spec_hit_dist_bytes};
+  for(int k = 0; k < 6; k++)
+    if(host[k] && have[k] < need[k])
+    {
+      h->err = "b200pt_read_dlss_guides: a destination is smaller than its plane (tile_rows x width in the plane's format)";
+      return B200PT_E_INVALID;
+    }
+  CK(cudaSetDevice(h->device));
+  {
+    const int frc = flushPending(h);
+    if(frc)
+      return frc;
+  }
+  for(int k = 0; k < 6; k++)
+    if(host[k])
+      CK(cudaMemcpyAsync(host[k], dev[k], need[k], cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return B200PT_OK;
+}
+
+int b200pt_get_dlss_guides_device(b200pt_t* h, b200pt_dlss_guides* out)
+{
+  if(!h || h->numPaths == 0 || !h->dDlss || !out)
+    return B200PT_E_INVALID;
+  void*  dev[6];
+  size_t bytes[6];
+  dlssPlanes(h, dev, bytes);
+  out->albedo = dev[0];
+  out->albedo_bytes = bytes[0];
+  out->spec_albedo = dev[1];
+  out->spec_albedo_bytes = bytes[1];
+  out->normal_roughness = dev[2];
+  out->normal_roughness_bytes = bytes[2];
+  out->motion = dev[3];
+  out->motion_bytes = bytes[3];
+  out->depth = dev[4];
+  out->depth_bytes = bytes[4];
+  out->spec_hit_dist = dev[5];
+  out->spec_hit_dist_bytes = bytes[5];
+  return B200PT_OK;
+}
+
 int b200pt_set_frame_batch(b200pt_t* h, int n)
 {
   if(!h || n < 1 || n > 64)
@@ -4243,10 +4505,15 @@ int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
     h->err = "b200pt_render_frame: the blurred HDR backplate (envBlur > 0: nvshaders' smoothHDRBlur, external) is not built";
     return B200PT_E_UNSUPPORTED;
   }
-  if(pc->flags & B200PT_PT_USE_DLSS)
+  if((pc->flags & B200PT_PT_USE_DLSS) && !h->dlss)
   {
-    h->err = "b200pt_render_frame: the DLSS variant (frame jitter, motion vectors, specular guides) is out of scope";
-    return B200PT_E_UNSUPPORTED;
+    h->err = "b200pt_render_frame: ePtUseDlss needs the DLSS guide images (b200pt_set_dlss_guides(h, 1) first)";
+    return B200PT_E_INVALID;
+  }
+  if((pc->flags & B200PT_PT_USE_DLSS) && pc->numSamples != 1)
+  {
+    h->err = "b200pt_render_frame: the DLSS variant renders one sample per frame (numSamples must be 1)";
+    return B200PT_E_INVALID;
   }
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && !h->guides)
   {
@@ -4260,6 +4527,14 @@ int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   }
   if(h->batch <= 1)
     return launchFrames(h, fi, pc, 1);
+  if(pc->flags & B200PT_PT_USE_DLSS)
+  {
+    // a DLSS frame runs alone: its jitter and camera change every frame, and it replaces the image
+    const int rc = flushPending(h);
+    if(rc)
+      return rc;
+    return launchFrames(h, fi, pc, 1);
+  }
   // frame batching: collect consecutive frames of a static camera (same frame constants; push constants that differ only by
   // the frame / sample counters advancing like the host loop advances them) and run them as one wavefront
   if(h->pendingCount > 0)
@@ -4320,6 +4595,9 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   F.pixels = h->numPaths;
   F.batch = count;
   F.numPaths = h->numPaths * (uint32_t)count;
+  F.prevObjectToWorld = ((pc->flags & B200PT_PT_USE_DLSS) && h->prevO2WValid) ? h->dPrevO2W : nullptr;
+  h->prevO2WValid = false;
+  h->renderedSinceUpdate = true;
 
   const int     laneIdx = (int)(h->frameSerial++ % (uint64_t)h->numLanes);
   b200pt::Lane& L = h->lanes[laneIdx];
@@ -4481,6 +4759,14 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   timed(tOther, [&] { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth); });
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && h->dGuide)
     timed(tOther, [&] { k_guide<<<gridWide, 256, 0, st>>>(L.P, F, h->dGuide); });
+  if((pc->flags & B200PT_PT_USE_DLSS) && h->dDlss)
+  {
+    void*  dev[6];
+    size_t bytes[6];
+    dlssPlanes(h, dev, bytes);
+    const DlssPlanes planes{(uint32_t*)dev[0], (uint2*)dev[1], (uint2*)dev[2], (uint32_t*)dev[3], (uint16_t*)dev[4], (uint16_t*)dev[5]};
+    timed(tOther, [&] { k_dlss_guides<<<gridWide, 256, 0, st>>>(L.P, F, planes); });
+  }
   CK(cudaEventRecord(L.freed, st));
   L.busy = true;
   h->lastLane = laneIdx;

@@ -119,6 +119,9 @@ struct FrameParams
   // frameCount and b * numSamples to totalSamples (what the host loop would have passed, src/renderer_pathtracer.cpp:1496-1574).
   uint32_t             pixels;    // tileRows * width
   int                  batch;     // >= 1
+  // DLSS frames: objectToWorld of every render node as the previous frame saw it (16 floats each, glm order), or null when no
+  // transform changed since that frame (pushConst.prevRenderNodeObjectToWorld, src/renderer_pathtracer.cpp:1553-1561)
+  const float*         prevObjectToWorld;
 };
 
 PT_D uint32_t pixelOf(const FrameParams& F, uint32_t i) { return F.batch > 1 ? i % F.pixels : i; }
@@ -160,7 +163,14 @@ struct PathState
   // albedo.xyz | roughness and normal.xyz | 1 (0: the primary ray missed), every value rounded through fp16 like the reference's float16_t fields
   float4*   guideA;
   float4*   guideN;
+  // DLSS scratch of the sample's first hit (null unless b200pt_set_dlss_guides): its previous-frame world position | 1 (primary
+  // miss: direction | 0), and GuideScratch's specular albedo + specular hit distance as binary16 bits (r | g << 16, b | dist << 16)
+  float4*   prevHit;
+  uint2*    dlssSpec;
 };
+
+// a DLSS frame (never batched) on a handle whose pools carry the DLSS scratch
+PT_D bool isDlssFrame(const PathState& P, const FrameParams& F) { return P.dlssSpec != nullptr && (F.pc.flags & B200PT_PT_USE_DLSS) != 0; }
 
 // flags word in misc.z
 enum : uint32_t
@@ -172,6 +182,7 @@ enum : uint32_t
   PF_SHADOW_VALID = 1u << 19,
   PF_SHADOW_INSIDE = 1u << 20, // TraceShadow(initialInside = true)
   PF_CATCHER = 1u << 21,       // the path sits on the shadow-catcher plane: the post stage runs handleShadowCatcher's second half
+  PF_SPEC_CAPTURE = 1u << 22,  // DLSS: GuideScratch::captureSpecularHit, the next Trace records the specular hit distance
 };
 
 struct Queues

@@ -77,6 +77,11 @@ class PathTracer:
         # OptiX-style guide image (albedo + camera-space normal of the first hit): set_guide_outputs(True) allocates it, every frame then
         # carries ePtUseOptixDenoiser (reference: the flag follows the denoiser selection, src/renderer_pathtracer.cpp:1547)
         self.ptUseOptixDenoiser = False
+        # DLSS variant (set_dlss_guides(True)): one jittered sample per frame, the image replaced, six guide images written.  The
+        # frame index restarts on resize (Dlss::notifyReset) and is the frame's frameCount (setupPushConstant :1514-1523).
+        self.ptUseDlss = False
+        self.m_dlssFrameIndex = 0
+        self.m_prevMVP = None          # GltfRenderer::m_prevMVP: the previous frame's viewProjMatrix (src/renderer.cpp:682, 703)
         self.ptPerformanceTarget = 1  # 0 interactive (60 FPS), 1 balanced (30), 2 quality (15), 3 max quality (10)
         self.last_frame_gpu_ms = None  # GPU time of the previous frame's path-trace section (the reference reads its profiler)
 
@@ -215,6 +220,7 @@ class PathTracer:
             self._ck(self._L.b200pt_resize(self._h, w, h, y0, rows), "b200pt_resize")
         self._size = (w, h)
         self._tile = (y0, rows)
+        self.m_dlssFrameIndex = 0
         resources.size = (w, h)
 
     MIN_SAMPLES_PER_PIXEL, MAX_SAMPLES_PER_PIXEL = 1, 100
@@ -254,16 +260,26 @@ class PathTracer:
                                      infinite_plane=s.useInfinitePlane, plane_distance=s.infinitePlaneDistance, plane_color=s.infinitePlaneBaseColor,
                                      plane_metallic=s.infinitePlaneMetallic, plane_roughness=s.infinitePlaneRoughness, shadow_catcher=s.isShadowCatcher,
                                      catcher_darkness=s.shadowCatcherDarkness)
+        if self.m_prevMVP is not None:
+            fi.prevMVP[:] = self.m_prevMVP
+        self.m_prevMVP = list(fi.viewProjMatrix)
+        num_samples = 1 if self.ptUseDlss else self.ptSamples
         pc = cam_mod.make_push_constant(resources.camera, h, frame_count=resources.frameCount,
-                                        total_samples=self.m_totalSamplesAccumulated, num_samples=self.ptSamples,
+                                        total_samples=self.m_totalSamplesAccumulated, num_samples=num_samples,
                                         max_depth=self.ptMaxDepth, firefly_clamp=self.ptFireflyClamp,
                                         tex_grad_scale=self.ptTexGradScale, aperture=self.ptAperture,
                                         focal_distance=None if self.ptAutoFocus else self.ptFocalDistance)
+        if self.ptUseDlss:
+            # setupPushConstant :1514-1523, 1543: the Halton index is the frameCount; ePtFirstFrame still follows resources.frameCount
+            self.m_dlssFrameIndex += 1
+            pc.frameCount = self.m_dlssFrameIndex
+            fi.jitter[:] = list(cam_mod.dlss_jitter(self.m_dlssFrameIndex))
+            pc.flags |= abi.PT_USE_DLSS
         if self.ptUseOptixDenoiser:
             pc.flags |= abi.PT_USE_OPTIX_DENOISER   # setupPushConstant :1547
         self.m_pushConst = pc
         self._ck(self._L.b200pt_render_frame(self._h, C.byref(fi), C.byref(pc)), "b200pt_render_frame")
-        self.m_totalSamplesAccumulated += self.ptSamples
+        self.m_totalSamplesAccumulated += num_samples
 
     # -- C-ABI passthroughs -------------------------------------------------------------------------
     def render_frame_raw(self, fi, pc):
@@ -313,6 +329,28 @@ class PathTracer:
         out = np.empty((rows, w, 4), np.float32)
         self._ck(self._L.b200pt_read_guide(self._h, out.ctypes.data_as(C.c_void_p), out.size), "b200pt_read_guide")
         return out[..., :3].copy(), out[..., 3].copy().view(np.uint32)
+
+    def set_dlss_guides(self, enable=True):
+        """b200pt_set_dlss_guides: the path pools carry the DLSS scratch; every frame then runs the DLSS variant"""
+        self._ck(self._L.b200pt_set_dlss_guides(self._h, 1 if enable else 0), "b200pt_set_dlss_guides")
+        self.ptUseDlss = bool(enable)
+
+    DLSS_PLANES = (("albedo", np.uint8, 4), ("spec_albedo", np.float16, 4), ("normal_roughness", np.float16, 4),
+                   ("motion", np.float16, 2), ("depth", np.float16, 1), ("spec_hit_dist", np.float16, 1))
+
+    def read_dlss_guides(self):
+        """the six DLSS guide images of the newest frame: albedo uint8 [rows, W, 4] (RGBA8 UNORM), spec_albedo and
+        normal_roughness float16 [rows, W, 4], motion float16 [rows, W, 2] (pixels), depth and spec_hit_dist float16 [rows, W]"""
+        w, _ = self._size
+        rows = self._tile[1]
+        out, g = {}, abi.DlssGuides()
+        for name, dt, ch in self.DLSS_PLANES:
+            a = np.empty((rows, w, ch) if ch > 1 else (rows, w), dt)
+            out[name] = a
+            setattr(g, name, a.ctypes.data)
+            setattr(g, name + "_bytes", a.nbytes)
+        self._ck(self._L.b200pt_read_dlss_guides(self._h, C.byref(g)), "b200pt_read_dlss_guides")
+        return out
 
     def read_selection(self):
         """gBuffers[eImgSelection] (object id per pixel, render node + 1, 0 = miss) and the NDC depth image, as the first
