@@ -287,7 +287,7 @@ const char* b200pt_last_error(const b200pt_t* h);
 /* Resources::sceneVk / sceneRtx hand-off; stands in for SceneVk::create (gltf_scene_vk.cpp:218-252)
  * + SceneRtx BLAS/TLAS build (gltf_scene_rtx.cpp:140-388) + PathTracer::onSceneInvalidated
  * (renderer_pathtracer.hpp:72).  Copies all arrays to HBM, builds the software wide BVH over the
- * world-space triangles of every visible render node, creates bindless texture objects. */
+ * world-space triangles of every visible render node, uploads the textures' mip chains as tiled texels. */
 int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* scene);
 
 /* ---- opacity micromaps (reference: src/gltf_scene_omm.{hpp,cpp} -- EXT_mesh_opacity_micromap uploaded as VK_EXT_opacity_micromap

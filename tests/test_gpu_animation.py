@@ -100,6 +100,11 @@ def test_animation_argument_checks(std_env):
         pt.set_animation([], [far])
     pt.set_animation(morphs, skins)
     pt.animate(*pose(2))
+    with pytest.raises(B200PTError):
+        pt.set_animation(morphs, [far])            # a refused set_animation leaves no tasks, not the previous ones
+    with pytest.raises(B200PTError):
+        pt.animate(*pose(1))
+    pt.set_animation(morphs, skins)
     pt.onSceneInvalidated(res)                     # a new scene drops the tasks
     with pytest.raises(B200PTError):
         pt.animate(*pose(1))
@@ -137,4 +142,9 @@ def test_node_hierarchy_on_the_device_matches_the_oracle(std_env, oracle_mod):
     bad[1], bad[2] = 2, 1                               # a cycle: no valid level order
     with pytest.raises(ValueError):
         pt.set_node_hierarchy(bad, mappings)
+    far = [(len(parents), mat, prim) for _, mat, prim in mappings]   # every render node mapped to a node out of range
+    with pytest.raises(B200PTError):
+        pt.set_node_hierarchy(parents, far)
+    with pytest.raises(B200PTError):
+        pt.update_node_matrices(glm(pose(1)))          # the refused hierarchy left none
     pt.onDetach(res)

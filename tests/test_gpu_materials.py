@@ -112,13 +112,11 @@ def test_thin_walled_scattering_material_is_not_truncated(std_env, oracle_mod):
     assert abs(img[..., :3].mean() / ref[..., :3].mean() - 1.0) <= 2e-2
 
 
-def test_malformed_scene_is_rejected(box_scene, std_env):
-    """Out-of-range indices / material ids / texture slots return B200PT_E_INVALID instead of reading out of bounds; so do
-    textures the device cannot sample like the reference: a side of 65536 or more (a 17th mip level, beyond the 16 the
-    device stores) and sampler enums getSampler does not map."""
+def malformed_scenes(box_scene):
+    """(what, scene): the box with one fault each -- an out-of-range index / material id / texture slot, or a texture the device
+    cannot sample like the reference (a side of 65536 or more, a sampler enum getSampler does not map)"""
     import copy
     from vk_gltf_renderer_b200 import synth
-    from vk_gltf_renderer_b200.renderer import B200PTError, PathTracer, Resources
     tex = {"tex_65536x1": (np.zeros((1, 65536, 4), np.uint8), {}), "tex_1x65536": (np.zeros((65536, 1, 4), np.uint8), {}),
            "wrap": (np.zeros((4, 4, 4), np.uint8), dict(wrapT=33069)), "mag": (np.zeros((4, 4, 4), np.uint8), dict(magFilter=9730)),
            "min": (np.zeros((4, 4, 4), np.uint8), dict(minFilter=9983))}
@@ -133,6 +131,17 @@ def test_malformed_scene_is_rejected(box_scene, std_env):
             scn.materials[0].pbrBaseColorTexture = 77
         else:
             scn.add_texture(tex[what][0], **tex[what][1])
+        yield what, scn
+
+
+def test_malformed_scene_is_rejected(box_scene, std_env):
+    """Out-of-range indices / material ids / texture slots return B200PT_E_INVALID instead of reading out of bounds; so do
+    textures the device cannot sample like the reference: a side of 65536 or more (a 17th mip level, beyond the 16 the
+    device stores) and sampler enums getSampler does not map."""
+    import copy
+    from vk_gltf_renderer_b200 import synth
+    from vk_gltf_renderer_b200.renderer import B200PTError, PathTracer, Resources
+    for what, scn in malformed_scenes(box_scene):
         pt = PathTracer(0)
         with pytest.raises(B200PTError, match="65536" if what.startswith("tex") else None):
             pt.onAttach(Resources(scene=scn, hdr_rgb=std_env, camera=scn.camera, size=(16, 16)))

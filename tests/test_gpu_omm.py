@@ -140,13 +140,14 @@ def test_special_indices_and_two_state_format(std_env, oracle_mod):
     assert moved[0] == 0 and moved[1] == 0 and moved[2] > 100 and moved[3] == 0
 
 
-def test_micromap_arguments_are_validated(std_env):
-    from vk_gltf_renderer_b200 import abi, omm, synth
-    from vk_gltf_renderer_b200.renderer import B200PTError
+def micromap_scene_and_bad_sets():
+    """one foliage layer and micromap sets the library must refuse: a subdivision level above 12, data beyond dataSize, a linkage to
+    a micromap, triangle or render primitive out of range, indices that do not cover the primitive"""
+    from vk_gltf_renderer_b200 import abi, synth
     scn = synth.synth_layers(layers=1, tex_size=32)
     pid = next(rn["renderPrimID"] for rn in scn.render_nodes if scn.materials[rn["materialID"]].alphaMode == 1)
     ntri = len(scn.render_prims[pid]["indices"])
-    bad = [
+    return scn, [
         dict(mm=[dict(data=np.zeros(1, np.uint8), triangles=np.array([(0, 13, 2)], abi.MICROMAP_TRIANGLE_DTYPE))], po=[dict(renderPrimID=pid, micromap=0, indices=np.zeros(ntri, np.int32))]),
         dict(mm=[dict(data=np.zeros(1, np.uint8), triangles=np.array([(0, 3, 2)], abi.MICROMAP_TRIANGLE_DTYPE))], po=[dict(renderPrimID=pid, micromap=0, indices=np.zeros(ntri, np.int32))]),
         dict(mm=[dict(data=np.zeros(16, np.uint8), triangles=np.array([(0, 3, 2)], abi.MICROMAP_TRIANGLE_DTYPE))], po=[dict(renderPrimID=pid, micromap=1, indices=np.zeros(ntri, np.int32))]),
@@ -154,6 +155,11 @@ def test_micromap_arguments_are_validated(std_env):
         dict(mm=[dict(data=np.zeros(16, np.uint8), triangles=np.array([(0, 3, 2)], abi.MICROMAP_TRIANGLE_DTYPE))], po=[dict(renderPrimID=pid, micromap=0, indices=np.zeros(1, np.int32))]),
         dict(mm=[dict(data=np.zeros(16, np.uint8), triangles=np.array([(0, 3, 2)], abi.MICROMAP_TRIANGLE_DTYPE))], po=[dict(renderPrimID=9999, micromap=0, indices=np.zeros(ntri, np.int32))]),
     ]
+
+
+def test_micromap_arguments_are_validated(std_env):
+    from vk_gltf_renderer_b200.renderer import B200PTError
+    scn, bad = micromap_scene_and_bad_sets()
     for b in bad:
         scn.micromaps, scn.prim_omms = b["mm"], b["po"]
         with pytest.raises(B200PTError):

@@ -32,6 +32,7 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <utility>
 #include <vector>
 
 #include "bvh.h"
@@ -1860,6 +1861,69 @@ __global__ void k_texture_lookup(DevScene S, const float* __restrict__ in, uint3
 // -------------------------------------------------------------------------------------------------
 // host side
 // -------------------------------------------------------------------------------------------------
+
+// Owner of the device allocations of one lifetime (the handle, a scene, a path pool, ...): they are freed together, by release() or
+// the destructor.  A call that fails returns nullptr and clears the CUDA error; the arena keeps the first failure for the caller's
+// report (`failed`), so a step may check once after several allocations.
+class DeviceArena
+{
+public:
+  DeviceArena() = default;
+  DeviceArena(const DeviceArena&) = delete;
+  DeviceArena& operator=(const DeviceArena&) = delete;
+  DeviceArena(DeviceArena&& o) noexcept : ptrs(std::move(o.ptrs)), error(o.error) { o.ptrs.clear(); }
+  DeviceArena& operator=(DeviceArena&& o) noexcept
+  {
+    release();
+    ptrs.swap(o.ptrs);
+    std::swap(error, o.error);
+    return *this;
+  }
+  ~DeviceArena() { release(); }
+
+  // n elements; at least one, so that every buffer has an address
+  template <typename T>
+  T* alloc(size_t n)
+  {
+    void* p = nullptr;
+    if(!keep(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T))))
+      return nullptr;
+    ptrs.push_back(p);
+    return static_cast<T*>(p);
+  }
+  // n elements copied from the host on `stream`; n == 0 gives one zeroed element
+  template <typename T>
+  T* upload(const T* src, size_t n, cudaStream_t stream)
+  {
+    T* d = alloc<T>(n);
+    if(d && !keep(n ? cudaMemcpyAsync(d, src, n * sizeof(T), cudaMemcpyHostToDevice, stream) : cudaMemsetAsync(d, 0, sizeof(T), stream)))
+      return nullptr;
+    return d;
+  }
+  void release()
+  {
+    for(void* p : ptrs)
+      cudaFree(p);
+    ptrs.clear();
+    error = cudaSuccess;
+  }
+  bool        ok() const { return error == cudaSuccess; }
+  cudaError_t takeError() { return std::exchange(error, cudaSuccess); }
+
+private:
+  bool keep(cudaError_t e)
+  {
+    if(e == cudaSuccess)
+      return true;
+    cudaGetLastError();
+    if(error == cudaSuccess)
+      error = e;
+    return false;
+  }
+  std::vector<void*> ptrs;
+  cudaError_t        error = cudaSuccess;
+};
+
 }  // namespace
 
 struct b200pt
@@ -1868,9 +1932,10 @@ struct b200pt
   cudaStream_t stream = nullptr;
   std::string  err;
   int          numSMs = 132;  // H100 SXM; b200pt_create reads the device's count
+  DeviceArena  mem;           // dStats, dLutSrgb, dTmHist and the lanes' counters and buckets
 
   // scene
-  std::vector<void*>  sceneAllocs;
+  DeviceArena         sceneMem;  // everything b200pt_set_scene uploads, and dPrevO2W
   const void*         treeBase = nullptr;  // the trees' node + triangle arrays (one allocation) and their size: the L2 window
   size_t              treeBytes = 0;
   int                 l2Window = 1;        // B200PT_L2_WINDOW=0: no persisting-L2 window over the trees
@@ -1934,24 +1999,31 @@ struct b200pt
   };
   std::vector<PrimHost>     primHost;
   ShadeRec*                 dShadeRecsW = nullptr;
-  std::vector<void*>        animAllocs;
-  std::vector<MorphTaskDev> morphTasks;
-  std::vector<SkinTaskDev>  skinTasks;
-  std::vector<uint32_t>     morphPrim, skinPrim;  // renderPrimID per task
-  float *                   dMorphWeights = nullptr, *dJointMats = nullptr, *dNormalMats = nullptr;
-  size_t                    numMorphWeights = 0, numJoints = 0;
+  struct Animation
+  {
+    DeviceArena               mem;
+    std::vector<MorphTaskDev> morphTasks;
+    std::vector<SkinTaskDev>  skinTasks;
+    std::vector<uint32_t>     morphPrim, skinPrim;  // renderPrimID per task
+    float *                   dMorphWeights = nullptr, *dJointMats = nullptr, *dNormalMats = nullptr;
+    size_t                    numMorphWeights = 0, numJoints = 0;
+  };
+  Animation anim;
   // node hierarchy on the device (b200pt_set_node_hierarchy / b200pt_update_node_matrices)
-  std::vector<void*>        graphAllocs;
-  std::vector<uint32_t>     levelOffsets;
-  uint32_t                  numGraphNodes = 0;
-  int *                     dParents = nullptr, *dTopo = nullptr;
-  float *                   dLocalMats = nullptr, *dWorldMats = nullptr, *dInstLocal = nullptr;
-  RenderNodeMapping*        dMappings = nullptr;
+  struct Hierarchy
+  {
+    DeviceArena           mem;
+    std::vector<uint32_t> levelOffsets;
+    uint32_t              numGraphNodes = 0;
+    int *                 dParents = nullptr, *dTopo = nullptr;
+    float *               dLocalMats = nullptr, *dWorldMats = nullptr, *dInstLocal = nullptr;
+    RenderNodeMapping*    dMappings = nullptr;
+  };
+  Hierarchy graph;
 
-  // env
-  float4* dEnv = nullptr;
-  uint2*  dEnvAccel = nullptr;
-  bool    haveEnv = false;
+  // env (S.envRgba / S.envAccel point into envMem)
+  DeviceArena envMem;
+  bool        haveEnv = false;
 
   // framebuffer + path pool
   int                width = 0, height = 0, tileY0 = 0, tileRows = 0;
@@ -1969,7 +2041,7 @@ struct b200pt
   float*             dPrevO2W = nullptr;
   bool               prevO2WValid = false;
   bool               renderedSinceUpdate = false;
-  uchar4*            dTonemapped = nullptr;  // gBuffers[eImgTonemapped] of this tile (b200pt_tonemap), in poolAllocs
+  uchar4*            dTonemapped = nullptr;  // gBuffers[eImgTonemapped] of this tile (b200pt_tonemap), in poolMem
   uint32_t*          dTmHist = nullptr;      // 256-bin log2-luminance histogram + the exposure factor behind it (allocated with the handle)
   uint32_t*          dSelect = nullptr;  // frame-0 outputs (gltf_pathtrace.slang:610-616): object id per pixel ...
   float*             dNdcDepth = nullptr;  // ... and NDC depth of the first hit
@@ -2001,13 +2073,13 @@ struct b200pt
   uint64_t           frameSerial = 0;
   int                lastLane = -1;
   cudaEvent_t        readDone[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-  std::vector<void*> poolAllocs;
+  DeviceArena        poolMem;
   // scratch pool of the ray-level API (b200pt_trace_closest / b200pt_trace_shadow run the production kernels on it)
   PathState          rayP{};
   uint32_t*          rayQ[3] = {nullptr, nullptr, nullptr};  // rays, any-hit, continuation
   uint32_t*          rayCounters = nullptr;                  // 8 words
   uint32_t           rayCapacity = 0;
-  std::vector<void*> rayAllocs;
+  DeviceArena        rayMem;
   DevStats*          dStats = nullptr;
   float*             dLutSrgb = nullptr;
 
@@ -2045,91 +2117,40 @@ namespace {
     }                                                                                                                                       \
   } while(0)
 
-template <typename T>
-int upload(b200pt* h, std::vector<void*>& owner, const T* src, size_t count, T** out)
+// the exit of a step whose arena failed: B200PT_E_NOMEM when the device is out of memory, B200PT_E_CUDA for any other error;
+// `what` names the buffer
+int failed(b200pt* h, DeviceArena& A, const char* what)
 {
-  *out = nullptr;
-  const size_t bytes = std::max<size_t>(count, 1) * sizeof(T);
-  void*        d = nullptr;
-  CK(cudaMalloc(&d, bytes));
-  owner.push_back(d);
-  if(count)
-    CK(cudaMemcpyAsync(d, src, count * sizeof(T), cudaMemcpyHostToDevice, h->stream));
-  else
-    CK(cudaMemsetAsync(d, 0, bytes, h->stream));
-  *out = (T*)d;
-  return 0;
+  const cudaError_t e = A.takeError();
+  if(e == cudaErrorMemoryAllocation)
+  {
+    h->err = std::string(what) + ": out of device memory";
+    return B200PT_E_NOMEM;
+  }
+  h->err = std::string(what) + ": " + cudaGetErrorString(e);
+  return B200PT_E_CUDA;
 }
 
-// the SoA arrays of one path pool (device_scene.cuh: PathState) for n paths
-int allocPathState(b200pt* h, std::vector<void*>& owner, size_t n, PathState& P)
+// the SoA arrays of one path pool (device_scene.cuh: PathState) for n paths; the caller checks A
+void allocPathState(const b200pt* h, DeviceArena& A, size_t n, PathState& P)
 {
   P = PathState{};
   float4** arrays[] = {&P.rayO, &P.rayD, &P.hit, &P.thr, &P.rad, &P.misc, reinterpret_cast<float4**>(&P.medium), &P.pixSum, &P.shO, &P.shD, &P.shC, &P.firstHit};
   for(float4** a : arrays)
-  {
-    void* d = nullptr;
-    if(cudaMalloc(&d, std::max<size_t>(n, 1) * 16) != cudaSuccess)
-    {
-      cudaGetLastError();
-      h->err = "path pool: out of device memory";
-      return B200PT_E_NOMEM;
-    }
-    owner.push_back(d);
-    *a = reinterpret_cast<float4*>(d);
-  }
+    *a = A.alloc<float4>(n);
   for(int k = 0; k < kCand; k++)
-  {
-    void* d = nullptr;
-    if(cudaMalloc(&d, std::max<size_t>(n, 1) * 16) != cudaSuccess)
-    {
-      cudaGetLastError();
-      h->err = "path pool: out of device memory";
-      return B200PT_E_NOMEM;
-    }
-    owner.push_back(d);
-    P.cand[k] = reinterpret_cast<float4*>(d);
-  }
-  void* d = nullptr;
-  if(cudaMalloc(&d, std::max<size_t>(n, 1) * sizeof(uint2)) != cudaSuccess)
-  {
-    cudaGetLastError();
-    h->err = "path pool: out of device memory";
-    return B200PT_E_NOMEM;
-  }
-  owner.push_back(d);
-  P.candInfo = reinterpret_cast<uint2*>(d);
+    P.cand[k] = A.alloc<float4>(n);
+  P.candInfo = A.alloc<uint2>(n);
   if(h->guides || h->dlss)
-    for(float4** a : {&P.guideA, &P.guideN})
-    {
-      void* g = nullptr;
-      if(cudaMalloc(&g, std::max<size_t>(n, 1) * 16) != cudaSuccess)
-      {
-        cudaGetLastError();
-        h->err = "path pool: out of device memory";
-        return B200PT_E_NOMEM;
-      }
-      owner.push_back(g);
-      *a = reinterpret_cast<float4*>(g);
-    }
+  {
+    P.guideA = A.alloc<float4>(n);
+    P.guideN = A.alloc<float4>(n);
+  }
   if(h->dlss)
   {
-    const size_t bytes[2] = {16, sizeof(uint2)};
-    void*        g[2] = {nullptr, nullptr};
-    for(int k = 0; k < 2; k++)
-    {
-      if(cudaMalloc(&g[k], std::max<size_t>(n, 1) * bytes[k]) != cudaSuccess)
-      {
-        cudaGetLastError();
-        h->err = "path pool: out of device memory";
-        return B200PT_E_NOMEM;
-      }
-      owner.push_back(g[k]);
-    }
-    P.prevHit = reinterpret_cast<float4*>(g[0]);
-    P.dlssSpec = reinterpret_cast<uint2*>(g[1]);
+    P.prevHit = A.alloc<float4>(n);
+    P.dlssSpec = A.alloc<uint2>(n);
   }
-  return B200PT_OK;
 }
 
 // Builds one compressed wide BVH over `m` of the scene's triangles ON THE DEVICE (lbvh.cuh) and brings it back in the host
@@ -2148,23 +2169,10 @@ int buildWideBvhGpu(b200pt* h, const float* dInRec, const uint32_t* dSubset, uin
   uint32_t M = 1;
   while(M < m)
     M <<= 1;
-  std::vector<void*> tmp;
-  auto               dalloc = [&](size_t bytes) -> void* {
-    void* p = nullptr;
-    if(cudaMalloc(&p, std::max<size_t>(bytes, 16)) != cudaSuccess)
-    {
-      cudaGetLastError();
-      return nullptr;
-    }
-    tmp.push_back(p);
-    return p;
-  };
-  auto cleanup = [&](int rc) {
-    for(void* p : tmp)
-      cudaFree(p);
-    if(rc)
-      h->err = "GPU BVH build failed (allocation or launch)";
-    return rc;
+  DeviceArena A;  // the build's scratch, freed on every return
+  auto        cudaFailed = [&]() {
+    h->err = "GPU BVH build failed (launch or copy)";
+    return B200PT_E_CUDA;
   };
   LbvhWork W{};
   W.m = m;
@@ -2172,27 +2180,26 @@ int buildWideBvhGpu(b200pt* h, const float* dInRec, const uint32_t* dSubset, uin
   W.inRec = dInRec;
   W.subset = dSubset;
   W.triBaseOffset = triBaseOffset;
-  W.primLo = (float4*)dalloc((size_t)m * 16);
-  W.primHi = (float4*)dalloc((size_t)m * 16);
-  W.keys = (unsigned long long*)dalloc((size_t)M * 8);
-  W.left = (int*)dalloc((size_t)m * 4);
-  W.right = (int*)dalloc((size_t)m * 4);
-  W.parentI = (int*)dalloc((size_t)m * 4);
-  W.parentL = (int*)dalloc((size_t)m * 4);
-  W.first = (uint32_t*)dalloc((size_t)m * 4);
-  W.last = (uint32_t*)dalloc((size_t)m * 4);
-  W.boxLo = (float4*)dalloc((size_t)m * 16);
-  W.boxHi = (float4*)dalloc((size_t)m * 16);
-  W.visits = (uint32_t*)dalloc((size_t)m * 4);
-  W.cbounds = (int*)dalloc(6 * 4);
-  W.nodes = (float*)dalloc(((size_t)m + 1) * 80);
-  W.tris = (float*)dalloc((size_t)m * 48);
-  W.triMeta = (uint32_t*)dalloc((size_t)m * 8);
-  W.counters = (uint32_t*)dalloc(4 * 4);
-  int2* queue[2] = {(int2*)dalloc(((size_t)m + 1) * 8), (int2*)dalloc(((size_t)m + 1) * 8)};
-  if(!W.primLo || !W.primHi || !W.keys || !W.left || !W.right || !W.parentI || !W.parentL || !W.first || !W.last || !W.boxLo || !W.boxHi || !W.visits || !W.cbounds
-     || !W.nodes || !W.tris || !W.triMeta || !W.counters || !queue[0] || !queue[1])
-    return cleanup(B200PT_E_NOMEM);
+  W.primLo = A.alloc<float4>(m);
+  W.primHi = A.alloc<float4>(m);
+  W.keys = A.alloc<unsigned long long>(M);
+  W.left = A.alloc<int>(m);
+  W.right = A.alloc<int>(m);
+  W.parentI = A.alloc<int>(m);
+  W.parentL = A.alloc<int>(m);
+  W.first = A.alloc<uint32_t>(m);
+  W.last = A.alloc<uint32_t>(m);
+  W.boxLo = A.alloc<float4>(m);
+  W.boxHi = A.alloc<float4>(m);
+  W.visits = A.alloc<uint32_t>(m);
+  W.cbounds = A.alloc<int>(6);
+  W.nodes = A.alloc<float>(((size_t)m + 1) * 20);
+  W.tris = A.alloc<float>((size_t)m * 12);
+  W.triMeta = A.alloc<uint32_t>((size_t)m * 2);
+  W.counters = A.alloc<uint32_t>(4);
+  int2* queue[2] = {A.alloc<int2>((size_t)m + 1), A.alloc<int2>((size_t)m + 1)};
+  if(!A.ok())
+    return failed(h, A, "GPU BVH build");
   cudaStream_t st = h->stream;
   const int    cbInit[6] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000};
   const uint32_t cnt0[4] = {1u, 0u, 0u, 0u};  // wide node 0 is the root
@@ -2201,7 +2208,7 @@ int buildWideBvhGpu(b200pt* h, const float* dInRec, const uint32_t* dSubset, uin
   ok = ok && cudaMemsetAsync(W.visits, 0, (size_t)m * 4, st) == cudaSuccess;
   ok = ok && cudaMemsetAsync(W.nodes, 0, ((size_t)m + 1) * 80, st) == cudaSuccess;
   if(!ok)
-    return cleanup(B200PT_E_CUDA);
+    return cudaFailed();
   const uint32_t gm = (m + 255) / 256, gM = (M + 255) / 256;
   k_lbvh_bounds<<<gm, 256, 0, st>>>(W);
   k_lbvh_morton<<<gM, 256, 0, st>>>(W);
@@ -2217,26 +2224,26 @@ int buildWideBvhGpu(b200pt* h, const float* dInRec, const uint32_t* dSubset, uin
   // collapse + emit, level by level
   const int2 rootEntry = make_int2(m >= 2 ? 0 : ~0, 0);
   if(cudaMemcpyAsync(queue[0], &rootEntry, sizeof(rootEntry), cudaMemcpyHostToDevice, st) != cudaSuccess)
-    return cleanup(B200PT_E_CUDA);
+    return cudaFailed();
   uint32_t count = 1, depth = 0;
   int      cur = 0;
   while(count)
   {
     const uint32_t zero = 0;
     if(cudaMemcpyAsync(&W.counters[2], &zero, 4, cudaMemcpyHostToDevice, st) != cudaSuccess)
-      return cleanup(B200PT_E_CUDA);
+      return cudaFailed();
     k_lbvh_emit<<<(count + 127) / 128, 128, 0, st>>>(W, queue[cur], count, queue[1 - cur]);
     h->kernelLaunches++;
     if(cudaMemcpyAsync(&count, &W.counters[2], 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-      return cleanup(B200PT_E_CUDA);
+      return cudaFailed();
     cur = 1 - cur;
     depth++;
     if(depth > 64)
-      return cleanup(B200PT_E_CUDA);
+      return cudaFailed();
   }
   uint32_t cnt[2] = {0, 0};
   if(cudaMemcpy(cnt, W.counters, 8, cudaMemcpyDeviceToHost) != cudaSuccess || cnt[1] != m || cnt[0] == 0 || cnt[0] > m + 1)
-    return cleanup(B200PT_E_CUDA);
+    return cudaFailed();
   out.numNodes = cnt[0];
   out.maxDepth = depth;
   out.nodes.resize((size_t)cnt[0] * 20);
@@ -2245,56 +2252,39 @@ int buildWideBvhGpu(b200pt* h, const float* dInRec, const uint32_t* dSubset, uin
   if(cudaMemcpy(out.nodes.data(), W.nodes, out.nodes.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess
      || cudaMemcpy(out.tris.data(), W.tris, out.tris.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess
      || cudaMemcpy(out.triMeta.data(), W.triMeta, out.triMeta.size() * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
-    return cleanup(B200PT_E_CUDA);
-  return cleanup(B200PT_OK);
+    return cudaFailed();
+  return B200PT_OK;
 }
 
 void freeRayPool(b200pt* h)
 {
-  for(void* p : h->rayAllocs)
-    cudaFree(p);
-  h->rayAllocs.clear();
+  h->rayMem.release();
   h->rayCapacity = 0;
 }
 
-void freeAnimation(b200pt* h)
-{
-  for(void* p : h->animAllocs)
-    cudaFree(p);
-  h->animAllocs.clear();
-  h->morphTasks.clear();
-  h->skinTasks.clear();
-  h->morphPrim.clear();
-  h->skinPrim.clear();
-  h->dMorphWeights = h->dJointMats = h->dNormalMats = nullptr;
-  h->numMorphWeights = h->numJoints = 0;
-}
-
-void freeHierarchy(b200pt* h)
-{
-  for(void* p : h->graphAllocs)
-    cudaFree(p);
-  h->graphAllocs.clear();
-  h->levelOffsets.clear();
-  h->numGraphNodes = 0;
-  h->dParents = h->dTopo = nullptr;
-  h->dLocalMats = h->dWorldMats = h->dInstLocal = nullptr;
-  h->dMappings = nullptr;
-}
-
+// drops the scene and everything built on it; h->S keeps only the environment and the sRGB table, h->tree[] is empty
 void freeScene(b200pt* h)
 {
-  cudaFree(h->dPrevO2W);
   h->dPrevO2W = nullptr;
   h->prevO2WValid = false;
   h->renderedSinceUpdate = false;
-  freeAnimation(h);
-  freeHierarchy(h);
-  for(void* p : h->sceneAllocs)
-    cudaFree(p);
-  h->sceneAllocs.clear();
+  h->anim = b200pt::Animation{};
+  h->graph = b200pt::Hierarchy{};
+  h->sceneMem.release();
   h->primHost.clear();
   h->dShadeRecsW = nullptr;
+  h->dNodesW = nullptr;
+  h->dPrimsW = nullptr;
+  h->numSceneNodes = 0;
+  for(auto& t : h->tree)
+    t = b200pt::TreeDev();
+  const DevScene old = h->S;
+  h->S = DevScene{};
+  h->S.envRgba = old.envRgba;
+  h->S.envAccel = old.envAccel;
+  h->S.envW = old.envW;
+  h->S.envH = old.envH;
+  h->S.lutSrgb = h->dLutSrgb;
   h->haveScene = false;
 }
 
@@ -2311,9 +2301,7 @@ void freePool(b200pt* h)
   for(int l = 0; l < b200pt::kMaxLanes; l++)
     h->lanes[l].busy = false;
   h->lastLane = -1;
-  for(void* p : h->poolAllocs)
-    cudaFree(p);
-  h->poolAllocs.clear();
+  h->poolMem.release();
   h->dAccumOwned = nullptr;
   h->dAccum = nullptr;
   h->dSelect = nullptr;
@@ -2482,6 +2470,18 @@ int checkDeviceErrors(b200pt* h)
   return B200PT_OK;
 }
 
+// the prologue of the entry points: the handle's device made current, the batched frames still pending launched and, with `sync`,
+// every stream idle, so that no frame in flight still reads what the call changes
+int enter(b200pt* h, bool sync)
+{
+  CK(cudaSetDevice(h->device));
+  if(const int rc = flushPending(h))
+    return rc;
+  if(sync)
+    syncAll(h);
+  return B200PT_OK;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -2531,8 +2531,8 @@ int b200pt_create(b200pt_t** out, int cuda_device)
   cudaDeviceProp prop{};
   need(cudaGetDeviceProperties(&prop, cuda_device));
   h->numSMs = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
-  need(cudaMalloc((void**)&h->dStats, sizeof(DevStats)));
-  if(ok)
+  h->dStats = h->mem.alloc<DevStats>(1);
+  if(h->dStats)
     need(cudaMemset(h->dStats, 0, sizeof(DevStats)));
   if(const char* e = getenv("B200PT_FRAMES_IN_FLIGHT"))
     h->numLanes = std::min(std::max(atoi(e), 1), (int)b200pt::kMaxLanes);
@@ -2561,9 +2561,9 @@ int b200pt_create(b200pt_t** out, int cuda_device)
     need(cudaStreamCreateWithFlags(&L.stream, cudaStreamNonBlocking));
     need(cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming));
     need(cudaEventCreateWithFlags(&L.freed, cudaEventDisableTiming));
-    need(cudaMalloc((void**)&L.dCounters, sizeof(uint32_t) * kCounterArrays * kMaxIters));
-    need(cudaMalloc((void**)&L.dBuckets, sizeof(uint32_t) * 2 * kSortMaxBuckets));
-    if(ok)
+    L.dCounters = h->mem.alloc<uint32_t>(kCounterArrays * kMaxIters);
+    L.dBuckets = h->mem.alloc<uint32_t>(2 * kSortMaxBuckets);
+    if(L.dBuckets)
       need(cudaMemset(L.dBuckets, 0, sizeof(uint32_t) * 2 * kSortMaxBuckets));
     need(cudaMallocHost((void**)&L.hCount, sizeof(uint32_t) * 4));
   }
@@ -2576,16 +2576,17 @@ int b200pt_create(b200pt_t** out, int cuda_device)
       lutS[i] = srgbToLinear((float)i / 255.0f);
       lutS[256 + i] = (float)i / 255.0f;
     }
-    need(cudaMalloc((void**)&h->dLutSrgb, sizeof(lutS)));
-    need(cudaMalloc((void**)&h->dTmHist, (kTmBins + 1) * sizeof(uint32_t)));  // histogram + the exposure factor (a float in the last word)
-    if(ok)
+    h->dLutSrgb = h->mem.alloc<float>(512);
+    h->dTmHist = h->mem.alloc<uint32_t>(kTmBins + 1);  // histogram + the exposure factor (a float in the last word)
+    if(h->dLutSrgb)
       need(cudaMemcpy(h->dLutSrgb, lutS, sizeof(lutS), cudaMemcpyHostToDevice));
   }
-  if(!ok)
+  if(!ok || !h->mem.ok())
   {
+    const int rc = h->mem.ok() ? B200PT_E_CUDA : B200PT_E_NOMEM;
     cudaGetLastError();  // clear the sticky-free error state for the next attempt
     b200pt_destroy(h);
-    return B200PT_E_CUDA;
+    return rc;
   }
   *out = h;
   return B200PT_OK;
@@ -2607,8 +2608,6 @@ void b200pt_destroy(b200pt_t* h)
   for(int l = 0; l < b200pt::kMaxLanes; l++)
   {
     b200pt::Lane& L = h->lanes[l];
-    cudaFree(L.dCounters);
-    cudaFree(L.dBuckets);
     if(L.hCount)
       cudaFreeHost(L.hCount);
     if(L.done)
@@ -2618,13 +2617,6 @@ void b200pt_destroy(b200pt_t* h)
     if(L.stream)
       cudaStreamDestroy(L.stream);
   }
-  if(h->dEnv)
-    cudaFree(h->dEnv);
-  if(h->dEnvAccel)
-    cudaFree(h->dEnvAccel);
-  cudaFree(h->dStats);
-  cudaFree(h->dLutSrgb);
-  cudaFree(h->dTmHist);
   for(auto& e : h->evPool)
   {
     cudaEventDestroy(e.a);
@@ -2635,274 +2627,259 @@ void b200pt_destroy(b200pt_t* h)
   if(h->timeline)
     fclose(h->timeline);
   cudaStreamDestroy(h->stream);
-  delete h;
+  delete h;  // (the arenas free the handle's and the environment's buffers)
 }
 
 const char* b200pt_last_error(const b200pt_t* h) { return h ? h->err.c_str() : "null handle"; }
 
 void* b200pt_stream(b200pt_t* h) { return h ? (void*)h->stream : nullptr; }
 
-int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
+}  // extern "C"
+namespace {
+
+// ---- b200pt_set_scene, step by step: validateScene, then steps that can only fail with E_NOMEM / E_CUDA, then commitScene ----
+
+// what b200pt_set_scene builds before it hands the scene to the handle
+struct SceneBuild
 {
-  if(!h || !s || s->numMaterials == 0 || (s->numRenderNodes && (!s->renderNodes || !s->renderPrimitives)))
-  {
-    if(h)
-      h->err = "b200pt_set_scene: invalid scene description";
+  DeviceArena                   mem;
+  DevScene                      S{};
+  b200pt_render_node*           nodesW = nullptr;  // == S.nodes, writable
+  ShadeRec*                     shadeRecsW = nullptr;  // == S.shadeRecs, writable
+  std::vector<b200pt::PrimHost> primHost;
+  std::vector<DevTex>           devTex;     // host copies of the texture records ...
+  std::vector<const uchar4*>    texLevel0;  // ... and their level-0 texels (device), for the alpha-triangle records
+  std::vector<FlatTri>          flat;
+  bool                          hasVolume = false, anyNonOpaque = false;
+  WideBvh                       bvh, bvhO, bvhA;
+  double                        bvhBuildMs = 0.0;
+  const void*                   treeBase = nullptr;
+  size_t                        treeBytes = 0;
+  b200pt::TreeDev               tree[3];
+  uint64_t                      nodeBytes = 0, triBytes = 0;
+  uint32_t                      ommTriangles = 0;
+};
+
+// the instance flags of a material's triangles (getInstanceFlag, src/gltf_scene_rtx.cpp:271-295)
+uint32_t triFlags(const b200pt_shade_material& m)
+{
+  uint32_t flags = 0;
+  if(m.transmissionFactor == 0.0f && m.alphaMode == 0 && m.diffuseTransmissionFactor == 0.0f)
+    flags |= TRI_OPAQUE;
+  if(m.doubleSided == 1 || m.thicknessFactor > 0.0f || m.transmissionFactor > 0.0f)
+    flags |= TRI_NOCULL;
+  return flags;
+}
+
+// every check of b200pt_set_scene, before its first allocation
+int validateScene(b200pt* h, const b200pt_scene_desc& s)
+{
+  auto refuse = [&](const std::string& msg) {
+    h->err = msg;
     return B200PT_E_INVALID;
-  }
-  CK(cudaSetDevice(h->device));
+  };
+  for(uint32_t i = 0; i < s.numMaterials; i++)
   {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
-  freeScene(h);
-  DevScene& S = h->S;
-  const int envW0 = S.envW, envH0 = S.envH;
-  S = DevScene{};
-  S.envRgba = h->dEnv;
-  S.envAccel = h->dEnvAccel;
-  S.envW = envW0;
-  S.envH = envH0;
-  S.lutSrgb = h->dLutSrgb;
-
-  // --- AoS tables: same bytes as the reference SSBOs ---
-  b200pt_render_node*    dNodes;
-  b200pt_shade_material* dMats;
-  b200pt_texture_info*   dTi;
-  b200pt_light*          dLights;
-  int                    rc;
-  if((rc = upload(h, h->sceneAllocs, s->renderNodes, s->numRenderNodes, &dNodes)))
-    return rc;
-  if((rc = upload(h, h->sceneAllocs, s->materials, s->numMaterials, &dMats)))
-    return rc;
-  if((rc = upload(h, h->sceneAllocs, s->textureInfos, s->numTextureInfos, &dTi)))
-    return rc;
-  if((rc = upload(h, h->sceneAllocs, s->lights, s->numLights, &dLights)))
-    return rc;
-  // which KHR_materials_* features do the scene's materials use (reference: src/scene_feature_detection.cpp)
-  {
-    uint32_t feat = s->numLights ? FEAT_LIGHTS : 0u;
-    for(uint32_t i = 0; i < s->numMaterials; i++)
+    const b200pt_shade_material& m = s.materials[i];
+    // the 22 texture slots index GltfTextureInfo[] (0 = none, shaders/gltf_scene_io.h.slang:196-219)
+    const uint16_t* slots = &m.pbrBaseColorTexture;
+    for(int k = 0; k < 22; k++)
+      if(slots[k] != 0 && slots[k] >= s.numTextureInfos)
+        return refuse("b200pt_set_scene: material texture slot beyond numTextureInfos");
+    if(m.retroreflectionFactor > 0.0f)
     {
-      const b200pt_shade_material& m = s->materials[i];
-      // the 22 texture slots index GltfTextureInfo[] (0 = none, shaders/gltf_scene_io.h.slang:196-219)
-      const uint16_t* slots = &m.pbrBaseColorTexture;
-      for(int k = 0; k < 22; k++)
-        if(slots[k] != 0 && slots[k] >= s->numTextureInfos)
-        {
-          h->err = "b200pt_set_scene: material texture slot beyond numTextureInfos";
-          return B200PT_E_INVALID;
-        }
-      if(m.retroreflectionFactor > 0.0f)
-      {
-        h->err = "b200pt_set_scene: KHR_materials_retroreflection is not built (its lobe lives in nvshaders, external to the reference tree)";
-        return B200PT_E_UNSUPPORTED;
-      }
-      if(m.transmissionFactor > 0.0f || m.transmissionTexture)
-        feat |= FEAT_TRANSMISSION;
-      if(m.thicknessFactor > 0.0f || m.thicknessTexture || m.multiscatterColorFactor[0] > 0.0f || m.multiscatterColorFactor[1] > 0.0f || m.multiscatterColorFactor[2] > 0.0f)
-        feat |= FEAT_VOLUME;
-      if(m.diffuseTransmissionFactor > 0.0f || m.diffuseTransmissionTexture)
-        feat |= FEAT_DIFFUSE_TRANSMISSION;
-      if(m.clearcoatFactor > 0.0f)
-        feat |= FEAT_CLEARCOAT;
-      if(m.sheenColorFactor[0] != 0.0f || m.sheenColorFactor[1] != 0.0f || m.sheenColorFactor[2] != 0.0f)
-        feat |= FEAT_SHEEN;
-      if(m.iridescenceFactor > 0.0f)
-        feat |= FEAT_IRIDESCENCE;
-      if(m.anisotropyStrength > 0.0f)
-        feat |= FEAT_ANISOTROPY;
-      if(m.pbrModel == 1)
-        feat |= FEAT_SPECGLOSS;
-    }
-    h->featureMask = feat;
-    h->leanShade = (feat & ~(uint32_t)FEAT_LEAN) == 0;
-  }
-  S.nodes = dNodes;
-  S.mats = dMats;
-  S.texInfos = dTi;
-  h->numTextureInfos = s->numTextureInfos;
-  S.lights = dLights;
-  S.numLights = (int)s->numLights;
-
-  // --- vertex data: separate attribute arrays per primitive, as SceneVk::createVertexBuffers ---
-  std::vector<DevPrim> prims(s->numRenderPrimitives);
-  for(uint32_t i = 0; i < s->numRenderPrimitives; i++)
-  {
-    const b200pt_render_primitive& p = s->renderPrimitives[i];
-    DevPrim&                       d = prims[i];
-    uint32_t*                      di;
-    float*                         df;
-    if((rc = upload(h, h->sceneAllocs, p.indices, (size_t)p.triangleCount * 3, &di)))
-      return rc;
-    d.idx = di;
-    if((rc = upload(h, h->sceneAllocs, p.positions, (size_t)p.vertexCount * 3, &df)))
-      return rc;
-    d.pos = df;
-    d.nrm = d.tan = d.uv0 = d.uv1 = nullptr;
-    d.col = nullptr;
-    if(p.normals)
-    {
-      if((rc = upload(h, h->sceneAllocs, p.normals, (size_t)p.vertexCount * 3, &df)))
-        return rc;
-      d.nrm = df;
-    }
-    if(p.tangents)
-    {
-      if((rc = upload(h, h->sceneAllocs, p.tangents, (size_t)p.vertexCount * 4, &df)))
-        return rc;
-      d.tan = df;
-    }
-    if(p.texCoords[0])
-    {
-      if((rc = upload(h, h->sceneAllocs, p.texCoords[0], (size_t)p.vertexCount * 2, &df)))
-        return rc;
-      d.uv0 = df;
-    }
-    if(p.texCoords[1])
-    {
-      if((rc = upload(h, h->sceneAllocs, p.texCoords[1], (size_t)p.vertexCount * 2, &df)))
-        return rc;
-      d.uv1 = df;
-    }
-    if(p.colors)
-    {
-      if((rc = upload(h, h->sceneAllocs, p.colors, (size_t)p.vertexCount, &di)))
-        return rc;
-      d.col = di;
+      h->err = "b200pt_set_scene: KHR_materials_retroreflection is not built (its lobe lives in nvshaders, external to the reference tree)";
+      return B200PT_E_UNSUPPORTED;
     }
   }
-  DevPrim* dPrims;
-  if((rc = upload(h, h->sceneAllocs, prims.data(), prims.size(), &dPrims)))
-    return rc;
-  S.prims = dPrims;
-  h->primHost.resize(s->numRenderPrimitives);
-  for(uint32_t i = 0; i < s->numRenderPrimitives; i++)
+  for(uint32_t i = 0; i < s.numTextures; i++)
   {
-    h->primHost[i].d = prims[i];
-    h->primHost[i].vertexCount = s->renderPrimitives[i].vertexCount;
-    h->primHost[i].triCount = s->renderPrimitives[i].triangleCount;
+    const b200pt_texture& t = s.textures[i];
+    if(t.width <= 0 || t.height <= 0 || !t.rgba8)
+      return refuse("texture without pixels");
+    // the device keeps 16 levels (packTiled): a side of 65536 or more has a 17th, which would be sampled as level 15
+    if(t.width >= 65536 || t.height >= 65536)
+      return refuse("texture " + std::to_string(i) + " is " + std::to_string(t.width) + "x" + std::to_string(t.height)
+                    + ": a side of 65536 or more needs more than the 16 mip levels the device stores");
+    // the glTF sampler enums getSampler maps (src/gltf_scene_vk.cpp:922-945; anything else throws there)
+    auto wrapOk = [](int m) { return m == 10497 || m == 33071 || m == 33648; };
+    auto filterOk = [](int f) { return f == -1 || f == 9728 || f == 9729 || (f >= 9984 && f <= 9987); };
+    if(!wrapOk(t.wrapS) || !wrapOk(t.wrapT) || !filterOk(t.magFilter) || !filterOk(t.minFilter))
+      return refuse("texture " + std::to_string(i) + " has a sampler enum outside glTF's (wrap " + std::to_string(t.wrapS) + "/" + std::to_string(t.wrapT)
+                    + ", filter " + std::to_string(t.magFilter) + "/" + std::to_string(t.minFilter) + ")");
   }
-
-  // --- textures ---
-  std::vector<DevTex> devTex(s->numTextures);
-  std::vector<const uchar4*> texLevel0(s->numTextures, nullptr);  // level-0 texels (device), for the alpha-triangle records
+  bool anyNonOpaque = false;  // as flattenInstances will find it
+  for(uint32_t n = 0; n < s.numRenderNodes; n++)
   {
-    for(uint32_t i = 0; i < s->numTextures; i++)
-    {
-      const b200pt_texture& t = s->textures[i];
-      if(t.width <= 0 || t.height <= 0 || !t.rgba8)
-      {
-        h->err = "texture without pixels";
-        return B200PT_E_INVALID;
-      }
-      // the device keeps 16 levels (packTiled): a side of 65536 or more has a 17th, which would be sampled as level 15
-      if(t.width >= 65536 || t.height >= 65536)
-      {
-        h->err = "texture " + std::to_string(i) + " is " + std::to_string(t.width) + "x" + std::to_string(t.height) + ": a side of 65536 or more needs more than the 16 mip levels the device stores";
-        return B200PT_E_INVALID;
-      }
-      // the glTF sampler enums getSampler maps (src/gltf_scene_vk.cpp:922-945; anything else throws there)
-      auto wrapOk = [](int m) { return m == 10497 || m == 33071 || m == 33648; };
-      auto filterOk = [](int f) { return f == -1 || f == 9728 || f == 9729 || (f >= 9984 && f <= 9987); };
-      if(!wrapOk(t.wrapS) || !wrapOk(t.wrapT) || !filterOk(t.magFilter) || !filterOk(t.minFilter))
-      {
-        h->err = "texture " + std::to_string(i) + " has a sampler enum outside glTF's (wrap " + std::to_string(t.wrapS) + "/" + std::to_string(t.wrapT)
-                 + ", filter " + std::to_string(t.magFilter) + "/" + std::to_string(t.minFilter) + ")";
-        return B200PT_E_INVALID;
-      }
-    }
-    std::vector<MipChain>    chains(s->numTextures);
-    std::atomic<uint32_t>    nextTex{0};
-    std::vector<std::thread> workers;
-    auto                     job = [&]() {
-      for(uint32_t i = nextTex.fetch_add(1); i < s->numTextures; i = nextTex.fetch_add(1))
-        buildMipChain(s->textures[i], chains[i]);
-    };
-    const unsigned nt = std::max(1u, std::min(std::thread::hardware_concurrency(), s->numTextures));
-    for(unsigned t = 1; t < nt; t++)
-      workers.emplace_back(job);
-    job();
-    for(auto& t : workers)
-      t.join();
-    // one allocation for all texels, one table of level offsets
-    std::vector<uint32_t> levelOfs((size_t)s->numTextures * 16, 0u);
-    std::vector<size_t>   texBase(s->numTextures, 0);
-    size_t                total = 0;
-    std::vector<std::vector<uint32_t>> packed(s->numTextures);
-    {
-      std::atomic<uint32_t>    nextPack{0};
-      std::vector<std::thread> packers;
-      auto                     pjob = [&]() {
-        for(uint32_t i = nextPack.fetch_add(1); i < s->numTextures; i = nextPack.fetch_add(1))
-          packTiled(chains[i], packed[i], &levelOfs[(size_t)i * 16]);
-      };
-      for(unsigned t = 1; t < nt; t++)
-        packers.emplace_back(pjob);
-      pjob();
-      for(auto& t : packers)
-        t.join();
-    }
-    for(uint32_t i = 0; i < s->numTextures; i++)
-    {
-      texBase[i] = total;
-      total += packed[i].size();
-    }
-    uint32_t* dTexels = nullptr;
-    uint32_t* dLevelOfs = nullptr;
-    CK(cudaMalloc((void**)&dTexels, std::max<size_t>(total, 1) * sizeof(uint32_t)));
-    h->sceneAllocs.push_back(dTexels);
-    for(uint32_t i = 0; i < s->numTextures; i++)
-      CK(cudaMemcpy(dTexels + texBase[i], packed[i].data(), packed[i].size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    if((rc = upload(h, h->sceneAllocs, levelOfs.data(), levelOfs.size(), &dLevelOfs)))
-      return rc;
-    for(uint32_t i = 0; i < s->numTextures; i++)
-    {
-      describeTexture(s->textures[i], chains[i], devTex[i]);
-      devTex[i].texels = reinterpret_cast<const uchar4*>(dTexels + texBase[i]);
-      texLevel0[i] = devTex[i].texels + levelOfs[(size_t)i * 16];
-      devTex[i].levelOfs = dLevelOfs + (size_t)i * 16;
-    }
-  }
-  DevTex* dTex;
-  if((rc = upload(h, h->sceneAllocs, devTex.data(), devTex.size(), &dTex)))
-    return rc;
-  S.textures = dTex;
-  S.numTextures = (int)s->numTextures;
-
-  // --- flatten instances to world space + build the wide BVH (TLAS/BLAS replacement) ---
-  std::vector<FlatTri> flat;
-  h->hasVolume = false;
-  for(uint32_t n = 0; n < s->numRenderNodes; n++)
-  {
-    if(s->renderNodeVisible && !s->renderNodeVisible[n])
+    if(s.renderNodeVisible && !s.renderNodeVisible[n])
       continue;
-    const b200pt_render_node& node = s->renderNodes[n];
-    if(node.renderPrimID < 0 || (uint32_t)node.renderPrimID >= s->numRenderPrimitives)
+    const b200pt_render_node& node = s.renderNodes[n];
+    if(node.renderPrimID < 0 || (uint32_t)node.renderPrimID >= s.numRenderPrimitives)
+      return refuse("render node references a missing primitive");
+    if(node.materialID >= (int)s.numMaterials)
+      return refuse("render node references a missing material");
+    if(s.renderPrimitives[node.renderPrimID].triangleCount && !(triFlags(s.materials[(uint32_t)std::max(0, node.materialID)]) & TRI_OPAQUE))
+      anyNonOpaque = true;
+  }
+  for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
+  {
+    const b200pt_render_primitive& p = s.renderPrimitives[i];
+    for(size_t k = 0; k < (size_t)p.triangleCount * 3; k++)
+      if(p.indices[k] >= p.vertexCount)
+        return refuse("b200pt_set_scene: index beyond the primitive's vertex count");
+  }
+  // the micromaps are linked only into scenes with non-opaque triangles (linkMicromaps)
+  if(anyNonOpaque)
+    for(const auto& po : h->primOmms)
     {
-      h->err = "render node references a missing primitive";
-      return B200PT_E_INVALID;
+      if(po.prim >= s.numRenderPrimitives)
+        return refuse("b200pt_set_scene: opacity micromap linked to a render primitive out of range");
+      const uint32_t nTri = s.renderPrimitives[po.prim].triangleCount;
+      if(po.hasIdx ? po.idx.size() < nTri : (uint64_t)po.base + nTri > h->omms[po.micromap].tris.size())
+        return refuse("b200pt_set_scene: opacity micromap does not cover its primitive's triangles");
     }
-    const b200pt_render_primitive& p = s->renderPrimitives[node.renderPrimID];
-    if(node.materialID >= (int)s->numMaterials)
-    {
-      h->err = "render node references a missing material";
-      return B200PT_E_INVALID;
-    }
-    const b200pt_shade_material&   m = s->materials[(uint32_t)std::max(0, node.materialID)];
-    uint32_t                       flags = 0;
-    if(m.transmissionFactor == 0.0f && m.alphaMode == 0 && m.diffuseTransmissionFactor == 0.0f)
-      flags |= TRI_OPAQUE;
-    if(m.doubleSided == 1 || m.thicknessFactor > 0.0f || m.transmissionFactor > 0.0f)
-      flags |= TRI_NOCULL;
+  return B200PT_OK;
+}
+
+// which KHR_materials_* features do the scene's materials use (reference: src/scene_feature_detection.cpp)
+uint32_t featureMaskOf(const b200pt_scene_desc& s)
+{
+  uint32_t feat = s.numLights ? FEAT_LIGHTS : 0u;
+  for(uint32_t i = 0; i < s.numMaterials; i++)
+  {
+    const b200pt_shade_material& m = s.materials[i];
+    if(m.transmissionFactor > 0.0f || m.transmissionTexture)
+      feat |= FEAT_TRANSMISSION;
+    if(m.thicknessFactor > 0.0f || m.thicknessTexture || m.multiscatterColorFactor[0] > 0.0f || m.multiscatterColorFactor[1] > 0.0f || m.multiscatterColorFactor[2] > 0.0f)
+      feat |= FEAT_VOLUME;
+    if(m.diffuseTransmissionFactor > 0.0f || m.diffuseTransmissionTexture)
+      feat |= FEAT_DIFFUSE_TRANSMISSION;
+    if(m.clearcoatFactor > 0.0f)
+      feat |= FEAT_CLEARCOAT;
+    if(m.sheenColorFactor[0] != 0.0f || m.sheenColorFactor[1] != 0.0f || m.sheenColorFactor[2] != 0.0f)
+      feat |= FEAT_SHEEN;
+    if(m.iridescenceFactor > 0.0f)
+      feat |= FEAT_IRIDESCENCE;
+    if(m.anisotropyStrength > 0.0f)
+      feat |= FEAT_ANISOTROPY;
+    if(m.pbrModel == 1)
+      feat |= FEAT_SPECGLOSS;
+  }
+  return feat;
+}
+
+// the AoS tables (same bytes as the reference SSBOs) and the vertex data: separate attribute arrays per primitive, as
+// SceneVk::createVertexBuffers
+int uploadTables(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  DeviceArena&       A = b.mem;
+  const cudaStream_t st = h->stream;
+  b.nodesW = A.upload(s.renderNodes, s.numRenderNodes, st);
+  b.S.nodes = b.nodesW;
+  b.S.mats = A.upload(s.materials, s.numMaterials, st);
+  b.S.texInfos = A.upload(s.textureInfos, s.numTextureInfos, st);
+  b.S.lights = A.upload(s.lights, s.numLights, st);
+  b.S.numLights = (int)s.numLights;
+  b.primHost.resize(s.numRenderPrimitives);
+  std::vector<DevPrim> prims(s.numRenderPrimitives);
+  for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
+  {
+    const b200pt_render_primitive& p = s.renderPrimitives[i];
+    const size_t                   nv = p.vertexCount;
+    DevPrim&                       d = prims[i];
+    d.idx = A.upload(p.indices, (size_t)p.triangleCount * 3, st);
+    d.pos = A.upload(p.positions, nv * 3, st);
+    d.nrm = p.normals ? A.upload(p.normals, nv * 3, st) : nullptr;
+    d.tan = p.tangents ? A.upload(p.tangents, nv * 4, st) : nullptr;
+    d.uv0 = p.texCoords[0] ? A.upload(p.texCoords[0], nv * 2, st) : nullptr;
+    d.uv1 = p.texCoords[1] ? A.upload(p.texCoords[1], nv * 2, st) : nullptr;
+    d.col = p.colors ? A.upload(p.colors, nv, st) : nullptr;
+    b.primHost[i].d = d;
+    b.primHost[i].vertexCount = p.vertexCount;
+    b.primHost[i].triCount = p.triangleCount;
+  }
+  b.S.prims = A.upload(prims.data(), prims.size(), st);
+  return A.ok() ? B200PT_OK : failed(h, A, "scene tables and vertex arrays");
+}
+
+// mip chains and tiling on host threads, one allocation for all texels, one table of level offsets, the DevTex records
+int uploadTextures(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  DeviceArena&             A = b.mem;
+  std::vector<MipChain>    chains(s.numTextures);
+  std::atomic<uint32_t>    nextTex{0};
+  std::vector<std::thread> workers;
+  auto                     job = [&]() {
+    for(uint32_t i = nextTex.fetch_add(1); i < s.numTextures; i = nextTex.fetch_add(1))
+      buildMipChain(s.textures[i], chains[i]);
+  };
+  const unsigned nt = std::max(1u, std::min(std::thread::hardware_concurrency(), s.numTextures));
+  for(unsigned t = 1; t < nt; t++)
+    workers.emplace_back(job);
+  job();
+  for(auto& t : workers)
+    t.join();
+  std::vector<uint32_t>              levelOfs((size_t)s.numTextures * 16, 0u);
+  std::vector<size_t>                texBase(s.numTextures, 0);
+  size_t                             total = 0;
+  std::vector<std::vector<uint32_t>> packed(s.numTextures);
+  {
+    std::atomic<uint32_t>    nextPack{0};
+    std::vector<std::thread> packers;
+    auto                     pjob = [&]() {
+      for(uint32_t i = nextPack.fetch_add(1); i < s.numTextures; i = nextPack.fetch_add(1))
+        packTiled(chains[i], packed[i], &levelOfs[(size_t)i * 16]);
+    };
+    for(unsigned t = 1; t < nt; t++)
+      packers.emplace_back(pjob);
+    pjob();
+    for(auto& t : packers)
+      t.join();
+  }
+  for(uint32_t i = 0; i < s.numTextures; i++)
+  {
+    texBase[i] = total;
+    total += packed[i].size();
+  }
+  uint32_t* dTexels = A.alloc<uint32_t>(total);
+  if(!dTexels)
+    return failed(h, A, "texels");
+  for(uint32_t i = 0; i < s.numTextures; i++)
+    CK(cudaMemcpy(dTexels + texBase[i], packed[i].data(), packed[i].size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+  const uint32_t* dLevelOfs = A.upload(levelOfs.data(), levelOfs.size(), h->stream);
+  if(!dLevelOfs)
+    return failed(h, A, "texture level offsets");
+  b.devTex.resize(s.numTextures);
+  b.texLevel0.resize(s.numTextures);
+  for(uint32_t i = 0; i < s.numTextures; i++)
+  {
+    describeTexture(s.textures[i], chains[i], b.devTex[i]);
+    b.devTex[i].texels = reinterpret_cast<const uchar4*>(dTexels + texBase[i]);
+    b.texLevel0[i] = b.devTex[i].texels + levelOfs[(size_t)i * 16];
+    b.devTex[i].levelOfs = dLevelOfs + (size_t)i * 16;
+  }
+  b.S.textures = A.upload(b.devTex.data(), b.devTex.size(), h->stream);
+  b.S.numTextures = (int)s.numTextures;
+  return b.S.textures ? B200PT_OK : failed(h, A, "texture records");
+}
+
+// every visible render node's triangles in world space (TLAS/BLAS replacement): flatten order is the global triangle id
+void flattenInstances(const b200pt_scene_desc& s, SceneBuild& b)
+{
+  for(uint32_t n = 0; n < s.numRenderNodes; n++)
+  {
+    if(s.renderNodeVisible && !s.renderNodeVisible[n])
+      continue;
+    const b200pt_render_node&      node = s.renderNodes[n];
+    const b200pt_render_primitive& p = s.renderPrimitives[node.renderPrimID];
+    const b200pt_shade_material&   m = s.materials[(uint32_t)std::max(0, node.materialID)];
+    const uint32_t                 flags = triFlags(m);
     // a path can take more than maxDepth wavefront iterations exactly when k_shade can scatter inside a medium: that
     // is gated on the medium's scatter coefficient (multiscatterColorFactor), not on thickness (makeVolumeMedium runs on
     // every transmission event, pathtrace_functions.h.slang:118-140, 605-672)
     if((m.transmissionFactor > 0.0f || m.transmissionTexture || m.diffuseTransmissionFactor > 0.0f || m.diffuseTransmissionTexture)
        && (m.multiscatterColorFactor[0] > 0.0f || m.multiscatterColorFactor[1] > 0.0f || m.multiscatterColorFactor[2] > 0.0f))
-      h->hasVolume = true;
+      b.hasVolume = true;
     const float* a = node.objectToWorld;
     const float  det = a[0] * (a[5] * a[10] - a[9] * a[6]) - a[4] * (a[1] * a[10] - a[9] * a[2]) + a[8] * (a[1] * a[6] - a[5] * a[2]);
     const bool   mirrored = det < 0.0f;
@@ -2912,11 +2889,6 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
       for(int k = 0; k < 3; k++)
       {
         const uint32_t vi = p.indices[t * 3 + k];
-        if(vi >= p.vertexCount)
-        {
-          h->err = "b200pt_set_scene: index beyond the primitive's vertex count";
-          return B200PT_E_INVALID;
-        }
         v[k] = xfPoint(a, f3(p.positions[vi * 3], p.positions[vi * 3 + 1], p.positions[vi * 3 + 2]));
       }
       FlatTri T;
@@ -2932,173 +2904,170 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
       T.v0[0] = v[0].x, T.v0[1] = v[0].y, T.v0[2] = v[0].z;
       T.e1[0] = e1.x, T.e1[1] = e1.y, T.e1[2] = e1.z;
       T.e2[0] = e2.x, T.e2[1] = e2.y, T.e2[2] = e2.z;
-      flat.push_back(T);
+      b.flat.push_back(T);
     }
   }
-  // ONE tree over every triangle (opaque and any-hit geometry alike: the per-triangle TRI_OPAQUE flag decides what a
-  // geometric hit means, traverse.cuh); the global triangle id (flatten order) is the tie-break key
-  std::vector<uint32_t> gids(flat.size());
-  bool                  anyNonOpaque = false;
+}
+
+// ONE tree over every triangle (opaque and any-hit geometry alike: the per-triangle TRI_OPAQUE flag decides what a geometric hit
+// means, traverse.cuh); the global triangle id (flatten order) is the tie-break key.  Closest-hit rays walk the merged tree;
+// shadow rays walk an opaque-only tree first (any hit ends the query, occluded rays never meet the foliage boxes) and the
+// non-opaque tree after it (traverse.cuh).  The three builds run in parallel.
+int buildTrees(b200pt* h, SceneBuild& b)
+{
+  const std::vector<FlatTri>& flat = b.flat;
+  std::vector<uint32_t>       gids(flat.size());
   for(uint32_t i = 0; i < (uint32_t)flat.size(); i++)
   {
     gids[i] = i;
-    anyNonOpaque = anyNonOpaque || !(flat[i].flags & TRI_OPAQUE);
+    b.anyNonOpaque = b.anyNonOpaque || !(flat[i].flags & TRI_OPAQUE);
   }
-  // closest-hit rays walk the merged tree; shadow rays walk an opaque-only tree first (any hit ends the query, occluded
-  // rays never meet the foliage boxes) and the non-opaque tree after it (traverse.cuh).  The three builds run in parallel.
-  WideBvh bvh, bvhO, bvhA;
+  std::vector<FlatTri>  flatO, flatA;
+  std::vector<uint32_t> gidO, gidA;
+  if(b.anyNonOpaque)
+    for(uint32_t i = 0; i < (uint32_t)flat.size(); i++)
+    {
+      if(flat[i].flags & TRI_OPAQUE)
+      {
+        flatO.push_back(flat[i]);
+        gidO.push_back(i);
+      }
+      else
+      {
+        flatA.push_back(flat[i]);
+        gidA.push_back(i);
+      }
+    }
+  const auto tBuild0 = std::chrono::steady_clock::now();
+  if(h->bvhBuilder == 1)
   {
-    std::vector<FlatTri>  flatO, flatA;
-    std::vector<uint32_t> gidO, gidA;
-    if(anyNonOpaque)
-      for(uint32_t i = 0; i < (uint32_t)flat.size(); i++)
-      {
-        if(flat[i].flags & TRI_OPAQUE)
-        {
-          flatO.push_back(flat[i]);
-          gidO.push_back(i);
-        }
-        else
-        {
-          flatA.push_back(flat[i]);
-          gidA.push_back(i);
-        }
-      }
-    const auto tBuild0 = std::chrono::steady_clock::now();
-    if(h->bvhBuilder == 1)
+    // device LBVH: the flattened records go up once (flatten order = global id order), the subsets as id lists
+    std::vector<float> rec(flat.size() * 12);
+    for(size_t i = 0; i < flat.size(); i++)
     {
-      // device LBVH: the flattened records go up once (flatten order = global id order), the subsets as id lists
-      std::vector<float> rec(flat.size() * 12);
-      for(size_t i = 0; i < flat.size(); i++)
-      {
-        const FlatTri& T = flat[i];
-        float*         R = &rec[i * 12];
-        const uint32_t w0 = T.rnode | (T.flags << 28), prim = T.prim, gid = (uint32_t)i;
-        memcpy(R, T.v0, 12);
-        memcpy(R + 3, &w0, 4);
-        memcpy(R + 4, T.e1, 12);
-        memcpy(R + 7, &prim, 4);
-        memcpy(R + 8, T.e2, 12);
-        memcpy(R + 11, &gid, 4);
-      }
-      float *   dRec = nullptr;
-      uint32_t *dO = nullptr, *dA = nullptr;
-      std::vector<void*> tmpAllocs;
-      if((rc = upload(h, tmpAllocs, rec.data(), rec.size(), &dRec)) == 0 && anyNonOpaque)
-      {
-        rc = upload(h, tmpAllocs, gidO.data(), gidO.size(), &dO);
-        if(!rc)
-          rc = upload(h, tmpAllocs, gidA.data(), gidA.size(), &dA);
-      }
+      const FlatTri& T = flat[i];
+      float*         R = &rec[i * 12];
+      const uint32_t w0 = T.rnode | (T.flags << 28), prim = T.prim, gid = (uint32_t)i;
+      memcpy(R, T.v0, 12);
+      memcpy(R + 3, &w0, 4);
+      memcpy(R + 4, T.e1, 12);
+      memcpy(R + 7, &prim, 4);
+      memcpy(R + 8, T.e2, 12);
+      memcpy(R + 11, &gid, 4);
+    }
+    DeviceArena     tmp;
+    const float*    dRec = tmp.upload(rec.data(), rec.size(), h->stream);
+    const uint32_t* dO = b.anyNonOpaque ? tmp.upload(gidO.data(), gidO.size(), h->stream) : nullptr;
+    const uint32_t* dA = b.anyNonOpaque ? tmp.upload(gidA.data(), gidA.size(), h->stream) : nullptr;
+    int             rc = tmp.ok() ? B200PT_OK : failed(h, tmp, "GPU BVH build input");
+    if(!rc)
+      rc = buildWideBvhGpu(h, dRec, nullptr, (uint32_t)flat.size(), 0u, b.bvh);
+    if(!rc && b.anyNonOpaque)
+    {
+      rc = buildWideBvhGpu(h, dRec, dO, (uint32_t)gidO.size(), 0u, b.bvhO);
       if(!rc)
-        rc = buildWideBvhGpu(h, dRec, nullptr, (uint32_t)flat.size(), 0u, bvh);
-      if(!rc && anyNonOpaque)
-      {
-        rc = buildWideBvhGpu(h, dRec, dO, (uint32_t)gidO.size(), 0u, bvhO);
-        if(!rc)
-          rc = buildWideBvhGpu(h, dRec, dA, (uint32_t)gidA.size(), (uint32_t)gidO.size(), bvhA);
-      }
-      cudaStreamSynchronize(h->stream);
-      for(void* p : tmpAllocs)
-        cudaFree(p);
-      if(rc)
-        return rc;
+        rc = buildWideBvhGpu(h, dRec, dA, (uint32_t)gidA.size(), (uint32_t)gidO.size(), b.bvhA);
     }
-    else
-    {
-      std::thread tO, tA;
-      if(anyNonOpaque)
-      {
-        tO = std::thread([&] { buildWideBvh(flatO, gidO, 0u, bvhO); });
-        tA = std::thread([&] { buildWideBvh(flatA, gidA, (uint32_t)flatO.size(), bvhA); });
-      }
-      buildWideBvh(flat, gids, 0u, bvh);
-      if(anyNonOpaque)
-      {
-        tO.join();
-        tA.join();
-      }
-    }
-    h->bvhBuildMs = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tBuild0).count();
+    cudaStreamSynchronize(h->stream);
+    if(rc)
+      return rc;
   }
-  // The node and triangle arrays of all three trees live in ONE allocation, so that a single L2 access-policy window can pin them
-  // (setTreeWindow below): the walks re-read these few tens of MB all the time while every bounce streams GBs of path state past them.
+  else
+  {
+    std::thread tO, tA;
+    if(b.anyNonOpaque)
+    {
+      tO = std::thread([&] { buildWideBvh(flatO, gidO, 0u, b.bvhO); });
+      tA = std::thread([&] { buildWideBvh(flatA, gidA, (uint32_t)flatO.size(), b.bvhA); });
+    }
+    buildWideBvh(flat, gids, 0u, b.bvh);
+    if(b.anyNonOpaque)
+    {
+      tO.join();
+      tA.join();
+    }
+  }
+  b.bvhBuildMs = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tBuild0).count();
+  return B200PT_OK;
+}
+
+// breadth-first level ranges of a tree (the builders emit level by level, so every level is one contiguous index range)
+std::vector<std::pair<uint32_t, uint32_t>> levelsOf(const WideBvh& t)
+{
+  std::vector<std::pair<uint32_t, uint32_t>> lv;
+  uint32_t                                   first = 0, count = 1;
+  while(count)
+  {
+    lv.push_back({first, count});
+    uint32_t next = 0;
+    for(uint32_t n = first; n < first + count; n++)
+    {
+      uint32_t w;
+      memcpy(&w, &t.nodes[(size_t)n * 20 + 3], 4);
+      next += (uint32_t)__builtin_popcount(w >> 24);
+    }
+    first += count;
+    count = next;
+  }
+  return lv;
+}
+
+// The node and triangle arrays of all three trees live in ONE allocation, so that a single L2 access-policy window can pin them
+// (setTreeWindow): the walks re-read these few tens of MB all the time while every bounce streams GBs of path state past them.
+// Also the trees' views for the refit (b200pt::TreeDev) with their level ranges and box scratch.
+int packTrees(b200pt* h, SceneBuild& b)
+{
+  DeviceArena&       A = b.mem;
+  const WideBvh &    bvh = b.bvh, &bvhO = b.bvhO, &bvhA = b.bvhA;
   std::vector<float> trisS, packed;
   size_t             offTris = 0, offNodesO = 0, offNodesA = 0, offTrisS = 0;
+  auto               place = [&](const std::vector<float>& v) {
+    const size_t at = packed.size();
+    packed.insert(packed.end(), v.begin(), v.end());
+    packed.resize((packed.size() + 31) & ~(size_t)31, 0.0f);  // 128-byte granules
+    return at;
+  };
+  place(bvh.nodes);
+  offTris = place(bvh.tris);
+  std::vector<uint32_t> metaS;
+  if(b.anyNonOpaque)
   {
-    auto place = [&](const std::vector<float>& v) {
-      const size_t at = packed.size();
-      packed.insert(packed.end(), v.begin(), v.end());
-      packed.resize((packed.size() + 31) & ~(size_t)31, 0.0f);  // 128-byte granules
-      return at;
-    };
-    place(bvh.nodes);
-    offTris = place(bvh.tris);
-    if(anyNonOpaque)
-    {
-      trisS = bvhO.tris;
-      trisS.insert(trisS.end(), bvhA.tris.begin(), bvhA.tris.end());
-      offNodesO = place(bvhO.nodes);
-      offNodesA = place(bvhA.nodes);
-      offTrisS = place(trisS);
-    }
+    trisS = bvhO.tris;
+    trisS.insert(trisS.end(), bvhA.tris.begin(), bvhA.tris.end());
+    offNodesO = place(bvhO.nodes);
+    offNodesA = place(bvhA.nodes);
+    offTrisS = place(trisS);
+    metaS = bvhO.triMeta;
+    metaS.insert(metaS.end(), bvhA.triMeta.begin(), bvhA.triMeta.end());
   }
-  float *   dPacked, *dBvhNodes, *dTris;
-  uint32_t* dMeta;
-  if((rc = upload(h, h->sceneAllocs, packed.data(), packed.size(), &dPacked)))
-    return rc;
-  dBvhNodes = dPacked;
-  dTris = dPacked + offTris;
-  h->treeBase = dPacked;
-  h->treeBytes = packed.size() * sizeof(float);
-  if((rc = upload(h, h->sceneAllocs, bvh.triMeta.data(), bvh.triMeta.size(), &dMeta)))
-    return rc;
-  S.bvh.nodes = reinterpret_cast<const float4*>(dBvhNodes);
-  S.bvh.tris = reinterpret_cast<const float4*>(dTris);
+  float* const    dPacked = A.upload(packed.data(), packed.size(), h->stream);
+  uint32_t* const dMeta = A.upload(bvh.triMeta.data(), bvh.triMeta.size(), h->stream);
+  uint32_t* const dMetaS = b.anyNonOpaque ? A.upload(metaS.data(), metaS.size(), h->stream) : nullptr;
+  if(!A.ok())
+    return failed(h, A, "trees");
+  b.treeBase = dPacked;
+  b.treeBytes = packed.size() * sizeof(float);
+  DevScene& S = b.S;
+  S.bvh.nodes = reinterpret_cast<const float4*>(dPacked);
+  S.bvh.tris = reinterpret_cast<const float4*>(dPacked + offTris);
   S.bvh.prmtPool = kPrmtPool;
   S.bvh.ommRef = nullptr;
   S.bvh.ommData = nullptr;
-  S.hasAlpha = anyNonOpaque ? 1 : 0;
+  S.hasAlpha = b.anyNonOpaque ? 1 : 0;
   S.triMeta = reinterpret_cast<const uint2*>(dMeta);
   S.bvhO = S.bvh;
   S.bvhA = S.bvh;
   S.triMetaS = S.triMeta;
-  // breadth-first level ranges of a tree (the builder emits level by level, so every level is one contiguous index range)
-  auto levelsOf = [](const WideBvh& t) {
-    std::vector<std::pair<uint32_t, uint32_t>> lv;
-    uint32_t                                   first = 0, count = 1;
-    while(count)
-    {
-      lv.push_back({first, count});
-      uint32_t next = 0;
-      for(uint32_t n = first; n < first + count; n++)
-      {
-        uint32_t w;
-        memcpy(&w, &t.nodes[(size_t)n * 20 + 3], 4);
-        next += (uint32_t)__builtin_popcount(w >> 24);
-      }
-      first += count;
-      count = next;
-    }
-    return lv;
-  };
-  for(auto& t : h->tree)
-    t = b200pt::TreeDev();
-  h->tree[0].nodes = dBvhNodes;
-  h->tree[0].tris = dTris;
-  h->tree[0].meta = reinterpret_cast<uint2*>(dMeta);
-  h->tree[0].numNodes = bvh.numNodes;
-  h->tree[0].numTriSlots = bvh.numTris;
-  h->tree[0].levels = levelsOf(bvh);
+  b.tree[0].nodes = dPacked;
+  b.tree[0].tris = dPacked + offTris;
+  b.tree[0].meta = reinterpret_cast<uint2*>(dMeta);
+  b.tree[0].numNodes = bvh.numNodes;
+  b.tree[0].numTriSlots = bvh.numTris;
+  b.tree[0].levels = levelsOf(bvh);
   uint64_t splitNodeBytes = 0, splitTriBytes = 0;
-  if(anyNonOpaque)
+  if(b.anyNonOpaque)
   {
-    std::vector<uint32_t> metaS(bvhO.triMeta);
-    metaS.insert(metaS.end(), bvhA.triMeta.begin(), bvhA.triMeta.end());
-    float *   dNodesO = dPacked + offNodesO, *dNodesA = dPacked + offNodesA, *dTrisS = dPacked + offTrisS;
-    uint32_t* dMetaS;
-    if((rc = upload(h, h->sceneAllocs, metaS.data(), metaS.size(), &dMetaS)))
-      return rc;
+    float *dNodesO = dPacked + offNodesO, *dNodesA = dPacked + offNodesA, *dTrisS = dPacked + offTrisS;
     S.bvhO.nodes = reinterpret_cast<const float4*>(dNodesO);
     S.bvhO.tris = reinterpret_cast<const float4*>(dTrisS);
     S.bvhA.nodes = reinterpret_cast<const float4*>(dNodesA);
@@ -3106,282 +3075,307 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
     S.triMetaS = reinterpret_cast<const uint2*>(dMetaS);
     splitNodeBytes = (bvhO.nodes.size() + bvhA.nodes.size()) * sizeof(float);
     splitTriBytes = trisS.size() * sizeof(float);
-    h->tree[1].nodes = dNodesO;
-    h->tree[1].tris = dTrisS;
-    h->tree[1].meta = reinterpret_cast<uint2*>(dMetaS);
-    h->tree[1].numNodes = bvhO.numNodes;
-    h->tree[1].numTriSlots = bvhO.numTris + bvhA.numTris;  // the shared array is refitted once, through this entry
-    h->tree[1].levels = levelsOf(bvhO);
-    h->tree[2].nodes = dNodesA;
-    h->tree[2].tris = dTrisS;
-    h->tree[2].meta = nullptr;
-    h->tree[2].numNodes = bvhA.numNodes;
-    h->tree[2].numTriSlots = 0;
-    h->tree[2].levels = levelsOf(bvhA);
+    b.tree[1].nodes = dNodesO;
+    b.tree[1].tris = dTrisS;
+    b.tree[1].meta = reinterpret_cast<uint2*>(dMetaS);
+    b.tree[1].numNodes = bvhO.numNodes;
+    b.tree[1].numTriSlots = bvhO.numTris + bvhA.numTris;  // the shared array is refitted once, through this entry
+    b.tree[1].levels = levelsOf(bvhO);
+    b.tree[2].nodes = dNodesA;
+    b.tree[2].tris = dTrisS;
+    b.tree[2].meta = nullptr;
+    b.tree[2].numNodes = bvhA.numNodes;
+    b.tree[2].numTriSlots = 0;
+    b.tree[2].levels = levelsOf(bvhA);
   }
-  for(auto& t : h->tree)
+  for(auto& t : b.tree)
     if(t.nodes)
-    {
-      CK(cudaMalloc((void**)&t.nodeBox, (size_t)std::max(t.numNodes, 1u) * 2 * sizeof(float4)));
-      h->sceneAllocs.push_back(t.nodeBox);
-    }
-  h->numSceneNodes = s->numRenderNodes;
-  h->dNodesW = dNodes;
-  h->dPrimsW = dPrims;
-  // ---- per-triangle attribute records for getHitState (device_scene.cuh: ShadeRec), per render primitive ----
+      t.nodeBox = A.alloc<float4>((size_t)std::max(t.numNodes, 1u) * 2);
+  if(!A.ok())
+    return failed(h, A, "refit boxes");
+  b.nodeBytes = bvh.nodes.size() * sizeof(float) + splitNodeBytes;
+  b.triBytes = bvh.tris.size() * sizeof(float) + splitTriBytes;
+  return B200PT_OK;
+}
+
+// per-triangle attribute records for getHitState (device_scene.cuh: ShadeRec), per render primitive, and the record and material
+// of every triangle slot of the merged tree
+int gatherShadeRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  DeviceArena&          A = b.mem;
+  std::vector<uint32_t> recBase(s.numRenderPrimitives, 0);
+  size_t                total = 0;
+  for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
   {
-    std::vector<uint32_t> recBase(s->numRenderPrimitives, 0);
-    size_t                total = 0;
-    for(uint32_t i = 0; i < s->numRenderPrimitives; i++)
+    recBase[i] = (uint32_t)total;
+    total += s.renderPrimitives[i].triangleCount;
+  }
+  std::vector<ShadeRec> recs(total);
+  for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
+  {
+    const b200pt_render_primitive& p = s.renderPrimitives[i];
+    for(uint32_t t = 0; t < p.triangleCount; t++)
     {
-      recBase[i] = (uint32_t)total;
-      total += s->renderPrimitives[i].triangleCount;
-    }
-    std::vector<ShadeRec> recs(total);
-    for(uint32_t i = 0; i < s->numRenderPrimitives; i++)
-    {
-      const b200pt_render_primitive& p = s->renderPrimitives[i];
-      for(uint32_t t = 0; t < p.triangleCount; t++)
+      ShadeRec& r = recs[recBase[i] + t];
+      float*    f = reinterpret_cast<float*>(&r);  // 48 floats, layout: device_scene.cuh ShadeRec
+      memset(f, 0, sizeof(ShadeRec));
+      const uint32_t flags = (p.normals ? 1u : 0u) | (p.texCoords[0] ? 2u : 0u) | (p.texCoords[1] ? 4u : 0u) | (p.colors ? 8u : 0u) | (p.tangents ? 16u : 0u);
+      memcpy(&f[3], &flags, 4);
+      uint32_t vi[3];
+      for(int c = 0; c < 3; c++)
       {
-        ShadeRec& r = recs[recBase[i] + t];
-        float*    f = reinterpret_cast<float*>(&r);  // 48 floats, layout: device_scene.cuh ShadeRec
-        memset(f, 0, sizeof(ShadeRec));
-        const uint32_t flags = (p.normals ? 1u : 0u) | (p.texCoords[0] ? 2u : 0u) | (p.texCoords[1] ? 4u : 0u) | (p.colors ? 8u : 0u) | (p.tangents ? 16u : 0u);
-        memcpy(&f[3], &flags, 4);
-        uint32_t vi[3];
+        vi[c] = p.indices[t * 3 + c];
+        memcpy(&f[c * 4], &p.positions[vi[c] * 3], 12);                 // v[0..2].xyz
+        if(p.normals)
+          memcpy(&f[12 + c * 4], &p.normals[vi[c] * 3], 12);            // v[3..5].xyz
+        if(p.colors)
+          memcpy(&f[7 + c * 4], &p.colors[vi[c]], 4);                   // v[1].w, v[2].w, v[3].w
+        if(p.tangents)
+          memcpy(&f[36 + c * 4], &p.tangents[vi[c] * 4], 16);           // v[9..11]
+      }
+      if(p.texCoords[0])
+      {
+        f[19] = p.texCoords[0][vi[0] * 2];                               // v[4].w
+        f[23] = p.texCoords[0][vi[0] * 2 + 1];                           // v[5].w
+        memcpy(&f[24], &p.texCoords[0][vi[1] * 2], 8);                   // v[6].xy
+        memcpy(&f[26], &p.texCoords[0][vi[2] * 2], 8);                   // v[6].zw
+      }
+      if(p.texCoords[1])
+      {
+        memcpy(&f[28], &p.texCoords[1][vi[0] * 2], 8);                   // v[7].xy
+        memcpy(&f[30], &p.texCoords[1][vi[1] * 2], 8);                   // v[7].zw
+        memcpy(&f[32], &p.texCoords[1][vi[2] * 2], 8);                   // v[8].xy
+      }
+    }
+  }
+  const WideBvh&        bvh = b.bvh;
+  std::vector<uint32_t> idxOfSlot(bvh.numTris, 0u);
+  for(uint32_t k = 0; k < bvh.numTris; k++)
+  {
+    uint32_t gid;
+    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
+    idxOfSlot[k] = recBase[s.renderNodes[b.flat[gid].rnode].renderPrimID] + b.flat[gid].prim;
+  }
+  std::vector<uint32_t> matOfSlot(bvh.numTris, 0u);
+  for(uint32_t k = 0; k < bvh.numTris; k++)
+  {
+    uint32_t gid;
+    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
+    matOfSlot[k] = (uint32_t)std::max(0, s.renderNodes[b.flat[gid].rnode].materialID);
+  }
+  b.shadeRecsW = A.upload(recs.data(), recs.size(), h->stream);
+  b.S.shadeRecs = b.shadeRecsW;
+  b.S.shadeIdx = A.upload(idxOfSlot.data(), idxOfSlot.size(), h->stream);
+  b.S.matOfSlot = A.upload(matOfSlot.data(), matOfSlot.size(), h->stream);
+  b.S.numMaterials = (int)s.numMaterials;
+  for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
+    b.primHost[i].recBase = recBase[i];
+  return A.ok() ? B200PT_OK : failed(h, A, "shade records");
+}
+
+// alpha-triangle records (device_scene.cuh: AlphaRec), one per non-opaque triangle in bvhA's leaf order
+int gatherAlphaRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  if(!b.anyNonOpaque)
+    return B200PT_OK;
+  DeviceArena&          A = b.mem;
+  const WideBvh &       bvh = b.bvh, &bvhA = b.bvhA;
+  const uint32_t        nA = bvhA.numTris;
+  std::vector<AlphaRec> recs(nA);
+  std::vector<uint32_t> recOfGid(b.flat.size(), 0xFFFFFFFFu);
+  for(uint32_t k = 0; k < nA; k++)
+  {
+    uint32_t gid;
+    memcpy(&gid, &bvhA.tris[(size_t)k * 12 + 11], 4);
+    recOfGid[gid] = k;
+    const FlatTri&                 T = b.flat[gid];
+    const b200pt_render_node&      node = s.renderNodes[T.rnode];
+    const b200pt_render_primitive& p = s.renderPrimitives[node.renderPrimID];
+    const b200pt_shade_material&   m = s.materials[(uint32_t)std::max(0, node.materialID)];
+    AlphaRec                       r{};
+    r.modeFlags = (uint32_t)m.alphaMode & 3u;
+    r.cutoff = m.alphaCutoff;
+    r.transmission = m.transmissionFactor;
+    const bool     specGloss = m.pbrModel == 1;
+    const uint16_t slot = specGloss ? m.pbrDiffuseTexture : m.pbrBaseColorTexture;
+    r.factor = specGloss ? m.pbrDiffuseFactor[3] : m.pbrBaseColorFactor[3];
+    const uint32_t i0 = p.indices[T.prim * 3], i1 = p.indices[T.prim * 3 + 1], i2 = p.indices[T.prim * 3 + 2];
+    if(slot > 0)
+    {
+      const b200pt_texture_info& ti = s.textureInfos[slot];
+      const float*               uv = ti.texCoord ? p.texCoords[1] : p.texCoords[0];
+      if(uv)
+      {
+        const uint32_t vi[3] = {i0, i1, i2};
         for(int c = 0; c < 3; c++)
         {
-          vi[c] = p.indices[t * 3 + c];
-          if(vi[c] >= p.vertexCount)
-          {
-            h->err = "b200pt_set_scene: index beyond the primitive's vertex count";
-            return B200PT_E_INVALID;
-          }
-          memcpy(&f[c * 4], &p.positions[vi[c] * 3], 12);                 // v[0..2].xyz
-          if(p.normals)
-            memcpy(&f[12 + c * 4], &p.normals[vi[c] * 3], 12);            // v[3..5].xyz
-          if(p.colors)
-            memcpy(&f[7 + c * 4], &p.colors[vi[c]], 4);                   // v[1].w, v[2].w, v[3].w
-          if(p.tangents)
-            memcpy(&f[36 + c * 4], &p.tangents[vi[c] * 4], 16);           // v[9..11]
-        }
-        if(p.texCoords[0])
-        {
-          f[19] = p.texCoords[0][vi[0] * 2];                               // v[4].w
-          f[23] = p.texCoords[0][vi[0] * 2 + 1];                           // v[5].w
-          memcpy(&f[24], &p.texCoords[0][vi[1] * 2], 8);                   // v[6].xy
-          memcpy(&f[26], &p.texCoords[0][vi[2] * 2], 8);                   // v[6].zw
-        }
-        if(p.texCoords[1])
-        {
-          memcpy(&f[28], &p.texCoords[1][vi[0] * 2], 8);                   // v[7].xy
-          memcpy(&f[30], &p.texCoords[1][vi[1] * 2], 8);                   // v[7].zw
-          memcpy(&f[32], &p.texCoords[1][vi[2] * 2], 8);                   // v[8].xy
+          r.uv[c * 2] = uv[vi[c] * 2];
+          r.uv[c * 2 + 1] = uv[vi[c] * 2 + 1];
         }
       }
+      if(ti.index >= 0 && (uint32_t)ti.index < s.numTextures)
+      {
+        const DevTex& dt = b.devTex[ti.index];
+        r.lv0 = b.texLevel0[ti.index];
+        r.w0 = dt.w0;
+        r.h0 = dt.h0;
+        r.wrap = ((uint32_t)dt.wrapS & 0xffffu) | ((uint32_t)dt.wrapT << 16);
+        if(dt.magLinear)
+          r.modeFlags |= 4u;
+      }
     }
-    std::vector<uint32_t> idxOfSlot(bvh.numTris, 0u);
-    for(uint32_t k = 0; k < bvh.numTris; k++)
+    if(p.colors)
     {
-      uint32_t gid;
-      memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
-      idxOfSlot[k] = recBase[s->renderNodes[flat[gid].rnode].renderPrimID] + flat[gid].prim;
+      r.modeFlags |= 8u;
+      r.colA = (p.colors[i0] >> 24) | ((p.colors[i1] >> 24) << 8) | ((p.colors[i2] >> 24) << 16);
     }
-    std::vector<uint32_t> matOfSlot(bvh.numTris, 0u);
-    for(uint32_t k = 0; k < bvh.numTris; k++)
-    {
-      uint32_t gid;
-      memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
-      matOfSlot[k] = (uint32_t)std::max(0, s->renderNodes[flat[gid].rnode].materialID);
-    }
-    ShadeRec* dRecs;
-    uint32_t *dIdx, *dMat;
-    if((rc = upload(h, h->sceneAllocs, recs.data(), recs.size(), &dRecs)))
-      return rc;
-    if((rc = upload(h, h->sceneAllocs, idxOfSlot.data(), idxOfSlot.size(), &dIdx)))
-      return rc;
-    if((rc = upload(h, h->sceneAllocs, matOfSlot.data(), matOfSlot.size(), &dMat)))
-      return rc;
-    S.shadeRecs = dRecs;
-    S.shadeIdx = dIdx;
-    h->dShadeRecsW = dRecs;
-    for(uint32_t i = 0; i < s->numRenderPrimitives; i++)
-      h->primHost[i].recBase = recBase[i];
-    S.matOfSlot = dMat;
-    S.numMaterials = (int)s->numMaterials;
+    recs[k] = r;
   }
+  std::vector<uint32_t> idxOfSlot(bvh.numTris, 0xFFFFFFFFu);
+  for(uint32_t k = 0; k < bvh.numTris; k++)
+  {
+    uint32_t gid;
+    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
+    idxOfSlot[k] = recOfGid[gid];
+  }
+  b.S.alphaRecs = A.upload(recs.data(), recs.size(), h->stream);
+  b.S.alphaIdx = A.upload(idxOfSlot.data(), idxOfSlot.size(), h->stream);
+  b.S.alphaBaseS = b.bvhO.numTris;
+  return A.ok() ? B200PT_OK : failed(h, A, "alpha records");
+}
 
-  // ---- alpha-triangle records (device_scene.cuh: AlphaRec), one per non-opaque triangle in bvhA's leaf order ----
-  S.alphaRecs = nullptr;
-  S.alphaIdx = nullptr;
-  S.alphaBaseS = 0;
-  if(anyNonOpaque)
+// opacity micromaps (omm.cuh): one reference word per triangle slot of the merged tree and of the shadow rays' arrays
+int linkMicromaps(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  if(!b.anyNonOpaque || h->primOmms.empty())
+    return B200PT_OK;
+  DeviceArena&          A = b.mem;
+  const WideBvh &       bvh = b.bvh, &bvhO = b.bvhO, &bvhA = b.bvhA;
+  std::vector<uint8_t>  data;
+  std::vector<uint32_t> dataBase(h->omms.size());
+  for(size_t m = 0; m < h->omms.size(); m++)
   {
-    const uint32_t        nA = bvhA.numTris;
-    std::vector<AlphaRec> recs(nA);
-    std::vector<uint32_t> recOfGid(flat.size(), 0xFFFFFFFFu);
-    for(uint32_t k = 0; k < nA; k++)
-    {
-      uint32_t gid;
-      memcpy(&gid, &bvhA.tris[(size_t)k * 12 + 11], 4);
-      recOfGid[gid] = k;
-      const FlatTri&                 T = flat[gid];
-      const b200pt_render_node&      node = s->renderNodes[T.rnode];
-      const b200pt_render_primitive& p = s->renderPrimitives[node.renderPrimID];
-      const b200pt_shade_material&   m = s->materials[(uint32_t)std::max(0, node.materialID)];
-      AlphaRec                       r{};
-      r.modeFlags = (uint32_t)m.alphaMode & 3u;
-      r.cutoff = m.alphaCutoff;
-      r.transmission = m.transmissionFactor;
-      const bool     specGloss = m.pbrModel == 1;
-      const uint16_t slot = specGloss ? m.pbrDiffuseTexture : m.pbrBaseColorTexture;
-      r.factor = specGloss ? m.pbrDiffuseFactor[3] : m.pbrBaseColorFactor[3];
-      const uint32_t i0 = p.indices[T.prim * 3], i1 = p.indices[T.prim * 3 + 1], i2 = p.indices[T.prim * 3 + 2];
-      if(slot > 0)
-      {
-        const b200pt_texture_info& ti = s->textureInfos[slot];
-        const float*               uv = ti.texCoord ? p.texCoords[1] : p.texCoords[0];
-        if(uv)
-        {
-          const uint32_t vi[3] = {i0, i1, i2};
-          for(int c = 0; c < 3; c++)
-          {
-            r.uv[c * 2] = uv[vi[c] * 2];
-            r.uv[c * 2 + 1] = uv[vi[c] * 2 + 1];
-          }
-        }
-        if(ti.index >= 0 && (uint32_t)ti.index < s->numTextures)
-        {
-          r.lv0 = texLevel0[ti.index];
-          r.w0 = devTex[ti.index].w0;
-          r.h0 = devTex[ti.index].h0;
-          r.wrap = ((uint32_t)devTex[ti.index].wrapS & 0xffffu) | ((uint32_t)devTex[ti.index].wrapT << 16);
-          if(devTex[ti.index].magLinear)
-            r.modeFlags |= 4u;
-        }
-      }
-      if(p.colors)
-      {
-        r.modeFlags |= 8u;
-        r.colA = (p.colors[i0] >> 24) | ((p.colors[i1] >> 24) << 8) | ((p.colors[i2] >> 24) << 16);
-      }
-      recs[k] = r;
-    }
-    std::vector<uint32_t> idxOfSlot(bvh.numTris, 0xFFFFFFFFu);
-    for(uint32_t k = 0; k < bvh.numTris; k++)
-    {
-      uint32_t gid;
-      memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
-      idxOfSlot[k] = recOfGid[gid];
-    }
-    AlphaRec* dRecs;
-    uint32_t* dIdx;
-    if((rc = upload(h, h->sceneAllocs, recs.data(), recs.size(), &dRecs)))
-      return rc;
-    if((rc = upload(h, h->sceneAllocs, idxOfSlot.data(), idxOfSlot.size(), &dIdx)))
-      return rc;
-    S.alphaRecs = dRecs;
-    S.alphaIdx = dIdx;
-    S.alphaBaseS = bvhO.numTris;
+    dataBase[m] = (uint32_t)data.size();
+    data.insert(data.end(), h->omms[m].data.begin(), h->omms[m].data.end());
   }
-  // ---- opacity micromaps (omm.cuh): one reference word per triangle slot of the merged tree and of the shadow rays' arrays ----
-  h->ommTriangles = 0;
-  if(anyNonOpaque && !h->primOmms.empty())
-  {
-    std::vector<uint8_t>  data;
-    std::vector<uint32_t> dataBase(h->omms.size());
-    for(size_t m = 0; m < h->omms.size(); m++)
-    {
-      dataBase[m] = (uint32_t)data.size();
-      data.insert(data.end(), h->omms[m].data.begin(), h->omms[m].data.end());
-    }
-    data.resize(data.size() + 4, 0);  // (never read: keeps the allocation non-empty)
-    std::vector<int> ommOfPrim(s->numRenderPrimitives, -1);
-    for(size_t k = 0; k < h->primOmms.size(); k++)
-    {
-      const auto& po = h->primOmms[k];
-      if(po.prim >= s->numRenderPrimitives)
-      {
-        h->err = "b200pt_set_scene: opacity micromap linked to a render primitive out of range";
-        return B200PT_E_INVALID;
-      }
-      const uint32_t nTri = s->renderPrimitives[po.prim].triangleCount;
-      if(po.hasIdx ? po.idx.size() < nTri : (uint64_t)po.base + nTri > h->omms[po.micromap].tris.size())
-      {
-        h->err = "b200pt_set_scene: opacity micromap does not cover its primitive's triangles";
-        return B200PT_E_INVALID;
-      }
-      ommOfPrim[po.prim] = (int)k;
-    }
-    uint32_t linked = 0;
-    auto     refOf = [&](uint32_t w0, uint32_t primTri) -> uint32_t {
-      const uint32_t unknown = pt::kOmmNoLookup | (uint32_t)pt::OMM_UNKNOWN;
-      if((w0 >> 28) & TRI_OPAQUE)
-        return unknown;  // FORCE_OPAQUE instance: the walk never asks
-      const int k = ommOfPrim[(uint32_t)s->renderNodes[w0 & 0x0fffffffu].renderPrimID];
-      if(k < 0)
-        return unknown;
-      const auto& po = h->primOmms[(size_t)k];
-      const int32_t idx = po.hasIdx ? po.idx[primTri] : (int32_t)primTri;
-      linked++;
-      if(idx == B200PT_OMM_INDEX_FULLY_TRANSPARENT)
-        return pt::kOmmNoLookup | (uint32_t)pt::OMM_TRANSPARENT;
-      if(idx == B200PT_OMM_INDEX_FULLY_OPAQUE)
-        return pt::kOmmNoLookup | (uint32_t)pt::OMM_OPAQUE;
-      if(idx < 0)
-        return unknown;
-      const b200pt_micromap_triangle& T = h->omms[po.micromap].tris[(size_t)idx + po.base];
-      return ((uint32_t)T.subdivisionLevel << 28) | (T.format == B200PT_OMM_FORMAT_4_STATE ? (1u << 27) : 0u) | (dataBase[po.micromap] + T.dataOffset);
-    };
-    std::vector<uint32_t> ref(bvh.numTris), refS((size_t)bvhO.numTris + bvhA.numTris, pt::kOmmNoLookup | (uint32_t)pt::OMM_UNKNOWN);
-    for(uint32_t k = 0; k < bvh.numTris; k++)
-      ref[k] = refOf(bvh.triMeta[(size_t)k * 2], bvh.triMeta[(size_t)k * 2 + 1]);
-    h->ommTriangles = linked;
-    for(uint32_t k = 0; k < bvhA.numTris; k++)
-      refS[(size_t)bvhO.numTris + k] = refOf(bvhA.triMeta[(size_t)k * 2], bvhA.triMeta[(size_t)k * 2 + 1]);
-    uint8_t*  dData;
-    uint32_t *dRef, *dRefS;
-    if((rc = upload(h, h->sceneAllocs, data.data(), data.size(), &dData)))
-      return rc;
-    if((rc = upload(h, h->sceneAllocs, ref.data(), ref.size(), &dRef)))
-      return rc;
-    if((rc = upload(h, h->sceneAllocs, refS.data(), refS.size(), &dRefS)))
-      return rc;
-    S.bvh.ommRef = dRef;
-    S.bvh.ommData = dData;
-    S.bvhA.ommRef = dRefS;
-    S.bvhA.ommData = dData;
-  }
-  h->nodeBytes = bvh.nodes.size() * sizeof(float) + splitNodeBytes;
-  h->triBytes = bvh.tris.size() * sizeof(float) + splitTriBytes;
-  h->numNodes = bvh.numNodes + (anyNonOpaque ? bvhO.numNodes + bvhA.numNodes : 0u);
-  h->numTris = bvh.numTris;
-  CK(cudaStreamSynchronize(h->stream));
+  data.resize(data.size() + 4, 0);  // (never read: keeps the allocation non-empty)
+  std::vector<int> ommOfPrim(s.numRenderPrimitives, -1);
+  for(size_t k = 0; k < h->primOmms.size(); k++)
+    ommOfPrim[h->primOmms[k].prim] = (int)k;
+  uint32_t linked = 0;
+  auto     refOf = [&](uint32_t w0, uint32_t primTri) -> uint32_t {
+    const uint32_t unknown = pt::kOmmNoLookup | (uint32_t)pt::OMM_UNKNOWN;
+    if((w0 >> 28) & TRI_OPAQUE)
+      return unknown;  // FORCE_OPAQUE instance: the walk never asks
+    const int k = ommOfPrim[(uint32_t)s.renderNodes[w0 & 0x0fffffffu].renderPrimID];
+    if(k < 0)
+      return unknown;
+    const auto&   po = h->primOmms[(size_t)k];
+    const int32_t idx = po.hasIdx ? po.idx[primTri] : (int32_t)primTri;
+    linked++;
+    if(idx == B200PT_OMM_INDEX_FULLY_TRANSPARENT)
+      return pt::kOmmNoLookup | (uint32_t)pt::OMM_TRANSPARENT;
+    if(idx == B200PT_OMM_INDEX_FULLY_OPAQUE)
+      return pt::kOmmNoLookup | (uint32_t)pt::OMM_OPAQUE;
+    if(idx < 0)
+      return unknown;
+    const b200pt_micromap_triangle& T = h->omms[po.micromap].tris[(size_t)idx + po.base];
+    return ((uint32_t)T.subdivisionLevel << 28) | (T.format == B200PT_OMM_FORMAT_4_STATE ? (1u << 27) : 0u) | (dataBase[po.micromap] + T.dataOffset);
+  };
+  std::vector<uint32_t> ref(bvh.numTris), refS((size_t)bvhO.numTris + bvhA.numTris, pt::kOmmNoLookup | (uint32_t)pt::OMM_UNKNOWN);
+  for(uint32_t k = 0; k < bvh.numTris; k++)
+    ref[k] = refOf(bvh.triMeta[(size_t)k * 2], bvh.triMeta[(size_t)k * 2 + 1]);
+  b.ommTriangles = linked;
+  for(uint32_t k = 0; k < bvhA.numTris; k++)
+    refS[(size_t)bvhO.numTris + k] = refOf(bvhA.triMeta[(size_t)k * 2], bvhA.triMeta[(size_t)k * 2 + 1]);
+  const uint8_t* dData = A.upload(data.data(), data.size(), h->stream);
+  b.S.bvh.ommRef = A.upload(ref.data(), ref.size(), h->stream);
+  b.S.bvh.ommData = dData;
+  b.S.bvhA.ommRef = A.upload(refS.data(), refS.size(), h->stream);
+  b.S.bvhA.ommData = dData;
+  return A.ok() ? B200PT_OK : failed(h, A, "micromap references");
+}
+
+// hands a built scene to the handle (after the last step that can fail)
+void commitScene(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  h->sceneMem = std::move(b.mem);
+  h->S = b.S;
+  h->numTextureInfos = s.numTextureInfos;
+  h->featureMask = featureMaskOf(s);
+  h->leanShade = (h->featureMask & ~(uint32_t)FEAT_LEAN) == 0;
+  h->primHost = std::move(b.primHost);
+  h->hasVolume = b.hasVolume;
+  h->bvhBuildMs = b.bvhBuildMs;
+  h->treeBase = b.treeBase;
+  h->treeBytes = b.treeBytes;
+  for(int t = 0; t < 3; t++)
+    h->tree[t] = std::move(b.tree[t]);
+  h->numSceneNodes = s.numRenderNodes;
+  h->dNodesW = b.nodesW;
+  h->dPrimsW = b.S.prims;
+  h->dShadeRecsW = b.shadeRecsW;
+  h->ommTriangles = b.ommTriangles;
+  h->nodeBytes = b.nodeBytes;
+  h->triBytes = b.triBytes;
+  h->numNodes = b.bvh.numNodes + (b.anyNonOpaque ? b.bvhO.numNodes + b.bvhA.numNodes : 0u);
+  h->numTris = b.bvh.numTris;
   h->haveScene = true;
-  // Persisting-L2 window over the trees on every stream that runs walks (cudaAccessPolicyWindow: lines of the window are kept, the
-  // path-state traffic around them is what gets evicted).  hitRatio shrinks when the trees are larger than the carve-out.
-  if(h->l2Window && h->treeBytes)
+}
+
+// Persisting-L2 window over the trees on every stream that runs walks (cudaAccessPolicyWindow: lines of the window are kept, the
+// path-state traffic around them is what gets evicted).  hitRatio shrinks when the trees are larger than the carve-out.
+void setTreeWindow(b200pt* h)
+{
+  if(!h->l2Window || !h->treeBytes)
+    return;
+  int maxPersist = 0, maxWindow = 0;
+  cudaDeviceGetAttribute(&maxPersist, cudaDevAttrMaxPersistingL2CacheSize, h->device);
+  cudaDeviceGetAttribute(&maxWindow, cudaDevAttrMaxAccessPolicyWindowSize, h->device);
+  if(maxPersist > 0 && maxWindow > 0)
   {
-    int maxPersist = 0, maxWindow = 0;
-    cudaDeviceGetAttribute(&maxPersist, cudaDevAttrMaxPersistingL2CacheSize, h->device);
-    cudaDeviceGetAttribute(&maxWindow, cudaDevAttrMaxAccessPolicyWindowSize, h->device);
-    if(maxPersist > 0 && maxWindow > 0)
-    {
-      const size_t carve = std::min<size_t>((size_t)maxPersist, std::max<size_t>(h->treeBytes, (size_t)1 << 20));
-      cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
-      cudaStreamAttrValue attr{};
-      attr.accessPolicyWindow.base_ptr = const_cast<void*>(h->treeBase);
-      attr.accessPolicyWindow.num_bytes = std::min<size_t>(h->treeBytes, (size_t)maxWindow);
-      attr.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)attr.accessPolicyWindow.num_bytes);
-      attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-      attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-      cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &attr);
-      for(int l = 0; l < b200pt::kMaxLanes; l++)
-        if(h->lanes[l].stream)
-          cudaStreamSetAttribute(h->lanes[l].stream, cudaStreamAttributeAccessPolicyWindow, &attr);
-      cudaGetLastError();  // (a refused window is not an error: the walks run without it)
-    }
+    const size_t carve = std::min<size_t>((size_t)maxPersist, std::max<size_t>(h->treeBytes, (size_t)1 << 20));
+    cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, carve);
+    cudaStreamAttrValue attr{};
+    attr.accessPolicyWindow.base_ptr = const_cast<void*>(h->treeBase);
+    attr.accessPolicyWindow.num_bytes = std::min<size_t>(h->treeBytes, (size_t)maxWindow);
+    attr.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)carve / (double)attr.accessPolicyWindow.num_bytes);
+    attr.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
+    attr.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
+    cudaStreamSetAttribute(h->stream, cudaStreamAttributeAccessPolicyWindow, &attr);
+    for(int l = 0; l < b200pt::kMaxLanes; l++)
+      if(h->lanes[l].stream)
+        cudaStreamSetAttribute(h->lanes[l].stream, cudaStreamAttributeAccessPolicyWindow, &attr);
+    cudaGetLastError();  // (a refused window is not an error: the walks run without it)
   }
+}
+
+}  // namespace
+extern "C" {
+
+int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
+{
+  if(!h || !s || s->numMaterials == 0 || (s->numRenderNodes && (!s->renderNodes || !s->renderPrimitives)))
+  {
+    if(h)
+      h->err = "b200pt_set_scene: invalid scene description";
+    return B200PT_E_INVALID;
+  }
+  if(const int rc = enter(h, true))
+    return rc;
+  freeScene(h);
+  SceneBuild b;
+  b.S = h->S;  // the environment and the sRGB table
+  int rc;
+  if((rc = validateScene(h, *s)) || (rc = uploadTables(h, *s, b)) || (rc = uploadTextures(h, *s, b)))
+    return rc;
+  flattenInstances(*s, b);
+  if((rc = buildTrees(h, b)) || (rc = packTrees(h, b)) || (rc = gatherShadeRecs(h, *s, b)) || (rc = gatherAlphaRecs(h, *s, b))
+     || (rc = linkMicromaps(h, *s, b)))
+    return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  commitScene(h, *s, b);
+  setTreeWindow(h);
   return B200PT_OK;
 }
 
@@ -3521,8 +3515,8 @@ static int snapshotPrevTransforms(b200pt_t* h)
 {
   if(!h->renderedSinceUpdate || h->numSceneNodes == 0)
     return B200PT_OK;
-  if(!h->dPrevO2W)
-    CK(cudaMalloc((void**)&h->dPrevO2W, (size_t)h->numSceneNodes * 16 * sizeof(float)));
+  if(!h->dPrevO2W && !(h->dPrevO2W = h->sceneMem.alloc<float>((size_t)h->numSceneNodes * 16)))
+    return failed(h, h->sceneMem, "previous transforms");
   k_snapshot_prev_transforms<<<(h->numSceneNodes + 255) / 256, 256, 0, h->stream>>>(h->dNodesW, h->dPrevO2W, h->numSceneNodes);
   h->kernelLaunches++;
   CK(cudaGetLastError());
@@ -3539,13 +3533,8 @@ int b200pt_update_transforms(b200pt_t* h, const b200pt_render_node* nodes, uint3
       h->err = "b200pt_update_transforms: needs the scene's render-node count (materials / primitives of the nodes must not change)";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   cudaStream_t st = h->stream;
   if(const int rc = snapshotPrevTransforms(h))
     return rc;
@@ -3561,16 +3550,10 @@ int b200pt_set_node_hierarchy(b200pt_t* h, const b200pt_node_hierarchy* g)
       h->err = "b200pt_set_node_hierarchy: needs a scene and a complete hierarchy description";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
-  freeHierarchy(h);
+  if(const int rc = enter(h, true))
+    return rc;
+  h->graph = b200pt::Hierarchy{};
   auto fail = [&](const char* msg) {
-    freeHierarchy(h);
     h->err = msg;
     return B200PT_E_INVALID;
   };
@@ -3602,56 +3585,51 @@ int b200pt_set_node_hierarchy(b200pt_t* h, const b200pt_node_hierarchy* g)
     if(m.nodeID < 0 || (uint32_t)m.nodeID >= g->numNodes || m.renderPrimID < 0 || (size_t)m.renderPrimID >= h->primHost.size() || m.materialID >= h->S.numMaterials)
       return fail("b200pt_set_node_hierarchy: render-node mapping out of range");
   }
-  int rc;
-  if((rc = upload(h, h->graphAllocs, g->parentIndices, g->numNodes, &h->dParents)))
-    return rc;
-  if((rc = upload(h, h->graphAllocs, g->topoNodeOrder, g->numNodes, &h->dTopo)))
-    return rc;
+  b200pt::Hierarchy  G;
+  const cudaStream_t st = h->stream;
+  G.dParents = G.mem.upload(g->parentIndices, g->numNodes, st);
+  G.dTopo = G.mem.upload(g->topoNodeOrder, g->numNodes, st);
   static_assert(sizeof(RenderNodeMapping) == sizeof(b200pt_render_node_mapping), "mapping layout");
-  if((rc = upload(h, h->graphAllocs, reinterpret_cast<const RenderNodeMapping*>(g->mappings), h->numSceneNodes, &h->dMappings)))
-    return rc;
-  if(g->instLocalMatrices && (rc = upload(h, h->graphAllocs, g->instLocalMatrices, (size_t)h->numSceneNodes * 16, &h->dInstLocal)))
-    return rc;
-  CK(cudaMalloc((void**)&h->dLocalMats, (size_t)g->numNodes * 16 * sizeof(float)));
-  h->graphAllocs.push_back(h->dLocalMats);
-  CK(cudaMalloc((void**)&h->dWorldMats, (size_t)g->numNodes * 16 * sizeof(float)));
-  h->graphAllocs.push_back(h->dWorldMats);
-  h->levelOffsets.assign(g->levelOffsets, g->levelOffsets + g->numLevels + 1);
-  h->numGraphNodes = g->numNodes;
-  CK(cudaStreamSynchronize(h->stream));
+  G.dMappings = G.mem.upload(reinterpret_cast<const RenderNodeMapping*>(g->mappings), h->numSceneNodes, st);
+  if(g->instLocalMatrices)
+    G.dInstLocal = G.mem.upload(g->instLocalMatrices, (size_t)h->numSceneNodes * 16, st);
+  G.dLocalMats = G.mem.alloc<float>((size_t)g->numNodes * 16);
+  G.dWorldMats = G.mem.alloc<float>((size_t)g->numNodes * 16);
+  if(!G.mem.ok())
+    return failed(h, G.mem, "node hierarchy");
+  G.levelOffsets.assign(g->levelOffsets, g->levelOffsets + g->numLevels + 1);
+  G.numGraphNodes = g->numNodes;
+  CK(cudaStreamSynchronize(st));
+  h->graph = std::move(G);
   return B200PT_OK;
 }
 
 int b200pt_update_node_matrices(b200pt_t* h, const float* local_matrices)
 {
-  if(!h || !h->haveScene || h->numGraphNodes == 0 || !local_matrices)
+  if(!h || !h->haveScene || h->graph.numGraphNodes == 0 || !local_matrices)
   {
     if(h)
       h->err = "b200pt_update_node_matrices: needs b200pt_set_node_hierarchy and the nodes' local matrices";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   cudaStream_t st = h->stream;
   if(const int rc = snapshotPrevTransforms(h))
     return rc;
-  CK(cudaMemcpyAsync(h->dLocalMats, local_matrices, (size_t)h->numGraphNodes * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
-  for(size_t l = 0; l + 1 < h->levelOffsets.size(); l++)
+  const b200pt::Hierarchy& G = h->graph;
+  CK(cudaMemcpyAsync(G.dLocalMats, local_matrices, (size_t)G.numGraphNodes * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
+  for(size_t l = 0; l + 1 < G.levelOffsets.size(); l++)
   {
-    const uint32_t count = h->levelOffsets[l + 1] - h->levelOffsets[l];
+    const uint32_t count = G.levelOffsets[l + 1] - G.levelOffsets[l];
     if(!count)
       continue;
-    k_propagate_level<<<(count + 255) / 256, 256, 0, st>>>(h->dLocalMats, h->dWorldMats, h->dParents, h->dTopo, h->levelOffsets[l], count);
+    k_propagate_level<<<(count + 255) / 256, 256, 0, st>>>(G.dLocalMats, G.dWorldMats, G.dParents, G.dTopo, G.levelOffsets[l], count);
     h->kernelLaunches++;
   }
   if(h->numSceneNodes)
   {
-    k_update_render_nodes<<<(h->numSceneNodes + 255) / 256, 256, 0, st>>>(h->dWorldMats, h->dMappings, h->dInstLocal, h->dNodesW, h->numSceneNodes);
+    k_update_render_nodes<<<(h->numSceneNodes + 255) / 256, 256, 0, st>>>(G.dWorldMats, G.dMappings, G.dInstLocal, h->dNodesW, h->numSceneNodes);
     h->kernelLaunches++;
   }
   CK(cudaGetLastError());
@@ -3666,20 +3644,16 @@ int b200pt_set_animation(b200pt_t* h, const b200pt_morph_task* morphs, uint32_t 
       h->err = "b200pt_set_animation: needs a scene (b200pt_set_scene first) and task arrays";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
-  freeAnimation(h);
+  if(const int rc = enter(h, true))
+    return rc;
+  h->anim = b200pt::Animation{};
   auto fail = [&](const char* msg) {
-    freeAnimation(h);
     h->err = msg;
     return B200PT_E_INVALID;
   };
-  int rc;
+  b200pt::Animation  a;
+  DeviceArena&       A = a.mem;
+  const cudaStream_t st = h->stream;
   for(uint32_t i = 0; i < num_morphs; i++)
   {
     const b200pt_morph_task& m = morphs[i];
@@ -3692,43 +3666,22 @@ int b200pt_set_animation(b200pt_t* h, const b200pt_morph_task* morphs, uint32_t 
     T.vertexCount = m.vertexCount;
     T.numTargets = m.numTargets;
     const size_t nv = m.vertexCount, nd = (size_t)m.numTargets * m.vertexCount * 3;
-    float*       d;
-    if((rc = upload(h, h->animAllocs, m.basePositions, nv * 3, &d)))
-      return rc;
-    T.basePos = d;
+    T.basePos = A.upload(m.basePositions, nv * 3, st);
     if(m.baseNormals && P.d.nrm)
-    {
-      if((rc = upload(h, h->animAllocs, m.baseNormals, nv * 3, &d)))
-        return rc;
-      T.baseNrm = d;
-    }
+      T.baseNrm = A.upload(m.baseNormals, nv * 3, st);
     if(m.baseTangents && P.d.tan)
-    {
-      if((rc = upload(h, h->animAllocs, m.baseTangents, nv * 4, &d)))
-        return rc;
-      T.baseTan = d;
-    }
-    if((rc = upload(h, h->animAllocs, m.positionDeltas, nd, &d)))
-      return rc;
-    T.dPos = d;
+      T.baseTan = A.upload(m.baseTangents, nv * 4, st);
+    T.dPos = A.upload(m.positionDeltas, nd, st);
     if(m.normalDeltas && T.baseNrm)
-    {
-      if((rc = upload(h, h->animAllocs, m.normalDeltas, nd, &d)))
-        return rc;
-      T.dNrm = d;
-    }
+      T.dNrm = A.upload(m.normalDeltas, nd, st);
     if(m.tangentDeltas && T.baseTan)
-    {
-      if((rc = upload(h, h->animAllocs, m.tangentDeltas, nd, &d)))
-        return rc;
-      T.dTan = d;
-    }
+      T.dTan = A.upload(m.tangentDeltas, nd, st);
     T.outPos = const_cast<float*>(P.d.pos);
     T.outNrm = const_cast<float*>(P.d.nrm);
     T.outTan = const_cast<float*>(P.d.tan);
-    h->numMorphWeights += m.numTargets;
-    h->morphTasks.push_back(T);
-    h->morphPrim.push_back(m.renderPrimID);
+    a.numMorphWeights += m.numTargets;
+    a.morphTasks.push_back(T);
+    a.morphPrim.push_back(m.renderPrimID);
   }
   for(uint32_t i = 0; i < num_skins; i++)
   {
@@ -3742,109 +3695,89 @@ int b200pt_set_animation(b200pt_t* h, const b200pt_morph_task* morphs, uint32_t 
     const size_t nv = k.vertexCount;
     T.vertexCount = k.vertexCount;
     T.numJoints = k.numJoints;
-    float* d;
-    int*   di;
-    if((rc = upload(h, h->animAllocs, k.basePositions, nv * 3, &d)))
-      return rc;
-    T.basePos = d;
+    T.basePos = A.upload(k.basePositions, nv * 3, st);
     if(k.baseNormals && P.d.nrm)
-    {
-      if((rc = upload(h, h->animAllocs, k.baseNormals, nv * 3, &d)))
-        return rc;
-      T.baseNrm = d;
-    }
+      T.baseNrm = A.upload(k.baseNormals, nv * 3, st);
     if(k.baseTangents && P.d.tan)
-    {
-      if((rc = upload(h, h->animAllocs, k.baseTangents, nv * 4, &d)))
-        return rc;
-      T.baseTan = d;
-    }
-    if((rc = upload(h, h->animAllocs, k.weights, nv * 4, &d)))
-      return rc;
-    T.weights = d;
-    if((rc = upload(h, h->animAllocs, k.joints, nv * 4, &di)))
-      return rc;
-    T.joints = di;
+      T.baseTan = A.upload(k.baseTangents, nv * 4, st);
+    T.weights = A.upload(k.weights, nv * 4, st);
+    T.joints = A.upload(k.joints, nv * 4, st);
     T.outPos = const_cast<float*>(P.d.pos);
     T.outNrm = const_cast<float*>(P.d.nrm);
     T.outTan = const_cast<float*>(P.d.tan);
-    h->numJoints += k.numJoints;
-    h->skinTasks.push_back(T);
-    h->skinPrim.push_back(k.renderPrimID);
+    a.numJoints += k.numJoints;
+    a.skinTasks.push_back(T);
+    a.skinPrim.push_back(k.renderPrimID);
   }
   // the per-frame buffers, sized once (createAnimationResources: totalJointMatBytes / totalNormalMatBytes / morph weights)
-  CK(cudaMalloc((void**)&h->dMorphWeights, std::max<size_t>(h->numMorphWeights, 1) * sizeof(float)));
-  h->animAllocs.push_back(h->dMorphWeights);
-  CK(cudaMalloc((void**)&h->dJointMats, std::max<size_t>(h->numJoints, 1) * 16 * sizeof(float)));
-  h->animAllocs.push_back(h->dJointMats);
-  CK(cudaMalloc((void**)&h->dNormalMats, std::max<size_t>(h->numJoints, 1) * 9 * sizeof(float)));
-  h->animAllocs.push_back(h->dNormalMats);
+  a.dMorphWeights = A.alloc<float>(a.numMorphWeights);
+  a.dJointMats = A.alloc<float>(a.numJoints * 16);
+  a.dNormalMats = A.alloc<float>(a.numJoints * 9);
+  if(!A.ok())
+    return failed(h, A, "animation");
   size_t wOfs = 0, jOfs = 0;
-  for(auto& T : h->morphTasks)
+  for(auto& T : a.morphTasks)
   {
-    T.weights = h->dMorphWeights + wOfs;
+    T.weights = a.dMorphWeights + wOfs;
     wOfs += T.numTargets;
   }
-  for(auto& T : h->skinTasks)
+  for(auto& T : a.skinTasks)
   {
-    T.jointMatrices = h->dJointMats + jOfs * 16;
-    T.normalMatrices = h->dNormalMats + jOfs * 9;
+    T.jointMatrices = a.dJointMats + jOfs * 16;
+    T.normalMatrices = a.dNormalMats + jOfs * 9;
     jOfs += T.numJoints;
   }
-  CK(cudaStreamSynchronize(h->stream));
+  CK(cudaStreamSynchronize(st));
+  h->anim = std::move(a);
   return B200PT_OK;
 }
 
 int b200pt_animate(b200pt_t* h, const float* morph_weights, const float* joint_matrices, const float* normal_matrices)
 {
-  if(!h || !h->haveScene || (h->morphTasks.empty() && h->skinTasks.empty()) || (h->numMorphWeights && !morph_weights)
-     || (h->numJoints && (!joint_matrices || !normal_matrices)))
+  if(!h || !h->haveScene || (h->anim.morphTasks.empty() && h->anim.skinTasks.empty()) || (h->anim.numMorphWeights && !morph_weights)
+     || (h->anim.numJoints && (!joint_matrices || !normal_matrices)))
   {
     if(h)
       h->err = "b200pt_animate: needs b200pt_set_animation and the per-frame weights / joint matrices / normal matrices of its tasks";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
-  cudaStream_t st = h->stream;
+  if(const int rc = enter(h, true))
+    return rc;
+  const b200pt::Animation& a = h->anim;
+  cudaStream_t             st = h->stream;
   // Phase 1 (gltf_scene_animation_vk.cpp:430-494): one upload of all per-frame data
-  if(h->numMorphWeights)
-    CK(cudaMemcpyAsync(h->dMorphWeights, morph_weights, h->numMorphWeights * sizeof(float), cudaMemcpyHostToDevice, st));
-  if(h->numJoints)
+  if(a.numMorphWeights)
+    CK(cudaMemcpyAsync(a.dMorphWeights, morph_weights, a.numMorphWeights * sizeof(float), cudaMemcpyHostToDevice, st));
+  if(a.numJoints)
   {
-    CK(cudaMemcpyAsync(h->dJointMats, joint_matrices, h->numJoints * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(h->dNormalMats, normal_matrices, h->numJoints * 9 * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(a.dJointMats, joint_matrices, a.numJoints * 16 * sizeof(float), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(a.dNormalMats, normal_matrices, a.numJoints * 9 * sizeof(float), cudaMemcpyHostToDevice, st));
   }
   // Phase 2 (:497-533): morph
   std::vector<uint8_t> touched(h->primHost.size(), 0), morphed(h->primHost.size(), 0);
-  for(size_t i = 0; i < h->morphTasks.size(); i++)
+  for(size_t i = 0; i < a.morphTasks.size(); i++)
   {
-    const MorphTaskDev& T = h->morphTasks[i];
+    const MorphTaskDev& T = a.morphTasks[i];
     if(T.numTargets == 0)
       continue;  // (:508) nothing to blend: the vertex buffers keep what they hold
     k_morph<<<(T.vertexCount + 255) / 256, 256, 0, st>>>(T);
     h->kernelLaunches++;
-    touched[h->morphPrim[i]] = morphed[h->morphPrim[i]] = 1;
+    touched[a.morphPrim[i]] = morphed[a.morphPrim[i]] = 1;
   }
   // Phase 3 (:536-582): skin; a primitive morphed above is skinned from its own (morphed) arrays
-  for(size_t i = 0; i < h->skinTasks.size(); i++)
+  for(size_t i = 0; i < a.skinTasks.size(); i++)
   {
-    SkinTaskDev T = h->skinTasks[i];
-    if(morphed[h->skinPrim[i]])
+    SkinTaskDev T = a.skinTasks[i];
+    if(morphed[a.skinPrim[i]])
     {
-      const DevPrim& P = h->primHost[h->skinPrim[i]].d;
+      const DevPrim& P = h->primHost[a.skinPrim[i]].d;
       T.basePos = P.pos;
       T.baseNrm = P.nrm ? P.nrm : T.baseNrm;
       T.baseTan = P.tan ? P.tan : T.baseTan;
     }
     k_skin<<<(T.vertexCount + 255) / 256, 256, 0, st>>>(T);
     h->kernelLaunches++;
-    touched[h->skinPrim[i]] = 1;
+    touched[a.skinPrim[i]] = 1;
   }
   // the per-triangle shade records of the touched primitives follow their vertex arrays
   for(size_t p = 0; p < touched.size(); p++)
@@ -3863,13 +3796,8 @@ int b200pt_set_environment(b200pt_t* h, const float* rgb, int w, int hh, float* 
 {
   if(!h || !rgb || w <= 0 || hh <= 0)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   const size_t n = (size_t)w * hh;
   // importance = texel solid angle * max(r,g,b); Vose alias table; pdf stored in alpha
   // (nvvk::HdrIbl, external to the reference tree; call site src/renderer.cpp:1994-1996)
@@ -3928,18 +3856,21 @@ int b200pt_set_environment(b200pt_t* h, const float* rgb, int w, int hh, float* 
     accel[i * 2] = alias[i];
     memcpy(&accel[i * 2 + 1], &q[i], 4);
   }
-  if(h->dEnv)
-    cudaFree(h->dEnv);
-  if(h->dEnvAccel)
-    cudaFree(h->dEnvAccel);
-  h->dEnv = nullptr;
-  h->dEnvAccel = nullptr;
-  CK(cudaMalloc((void**)&h->dEnv, n * sizeof(float4)));
-  CK(cudaMalloc((void**)&h->dEnvAccel, n * sizeof(uint2)));
-  CK(cudaMemcpy(h->dEnv, rgba.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(h->dEnvAccel, accel.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
-  h->S.envRgba = h->dEnv;
-  h->S.envAccel = h->dEnvAccel;
+  // the old environment goes first (peak memory stays one environment); until the new one is complete there is none
+  h->envMem.release();
+  h->haveEnv = false;
+  h->S.envRgba = nullptr;
+  h->S.envAccel = nullptr;
+  DeviceArena   A;
+  float4* const dEnv = A.alloc<float4>(n);
+  uint2* const  dEnvAccel = A.alloc<uint2>(n);
+  if(!A.ok())
+    return failed(h, A, "environment");
+  CK(cudaMemcpy(dEnv, rgba.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(dEnvAccel, accel.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
+  h->envMem = std::move(A);
+  h->S.envRgba = dEnv;
+  h->S.envAccel = dEnvAccel;
   h->S.envW = w;
   h->S.envH = hh;
   h->haveEnv = true;
@@ -3956,103 +3887,63 @@ int b200pt_resize(b200pt_t* h, int width, int height, int tile_y0, int tile_rows
       h->err = "b200pt_resize: invalid extent / tile";
     return B200PT_E_INVALID;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   freePool(h);
   const size_t n = (size_t)width * tile_rows;          // pixels of the tile: image-sized buffers
   const size_t nPool = n * (size_t)std::max(h->batch, 1);  // path slots per lane
   // nothing of the handle's geometry is committed before every allocation has succeeded: a failed resize leaves
   // numPaths == 0 and null pointers, so later calls fail their guards instead of touching freed memory
-  auto fail = [&](int rc) {
-    freePool(h);
-    return rc;
-  };
+  DeviceArena A;
+  PathState   P[b200pt::kMaxLanes];
+  uint32_t*   dQ[b200pt::kMaxLanes][6] = {};
   for(int l = 0; l < h->numLanes; l++)
   {
-    b200pt::Lane& L = h->lanes[l];
-    const int     rc = allocPathState(h, h->poolAllocs, nPool, L.P);
-    if(rc)
-      return fail(rc);
+    allocPathState(h, A, nPool, P[l]);
     for(int k = 0; k < 6; k++)
-    {
-      if(cudaMalloc((void**)&L.dQ[k], nPool * sizeof(uint32_t)) != cudaSuccess)
-      {
-        cudaGetLastError();
-        L.dQ[k] = nullptr;
-        h->err = "path pool: out of device memory";
-        return fail(B200PT_E_NOMEM);
-      }
-      h->poolAllocs.push_back(L.dQ[k]);
-    }
+      dQ[l][k] = A.alloc<uint32_t>(nPool);
   }
-  if(cudaMalloc((void**)&h->dAccumOwned, n * 16) != cudaSuccess)
+  if(!A.ok())
+    return failed(h, A, "path pool");
+  float4* const accum = A.alloc<float4>(n);
+  if(!accum)
+    return failed(h, A, "accumulation image");
+  uint32_t* const select = A.alloc<uint32_t>(n);
+  if(!select)
+    return failed(h, A, "selection image");
+  float* const ndcDepth = A.alloc<float>(n);
+  if(!ndcDepth)
+    return failed(h, A, "depth image");
+  float4* const  guide = h->guides ? A.alloc<float4>(n) : nullptr;
+  if(h->guides && !guide)
+    return failed(h, A, "guide image");
+  const size_t   dlssBytes = n * kDlssBytesPerPixel + 6 * 256;
+  uint8_t* const dlss = h->dlss ? A.alloc<uint8_t>(dlssBytes) : nullptr;
+  if(h->dlss && !dlss)
+    return failed(h, A, "DLSS guide images");
+  uchar4* const tonemapped = A.alloc<uchar4>(n);
+  if(!tonemapped)
+    return failed(h, A, "tonemapped image");
+  const cudaStream_t st = h->stream;
+  if((guide && cudaMemsetAsync(guide, 0, n * 16, st) != cudaSuccess) || (dlss && cudaMemsetAsync(dlss, 0, dlssBytes, st) != cudaSuccess)
+     || cudaMemsetAsync(select, 0, n * 4, st) != cudaSuccess || cudaMemsetAsync(ndcDepth, 0, n * 4, st) != cudaSuccess
+     || cudaMemsetAsync(accum, 0, n * 16, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
   {
-    cudaGetLastError();
-    h->err = "accumulation image: out of device memory";
-    return fail(B200PT_E_NOMEM);
+    h->err = "b200pt_resize: clearing the new images failed";
+    return B200PT_E_CUDA;
   }
-  h->poolAllocs.push_back(h->dAccumOwned);
-  if(cudaMalloc((void**)&h->dSelect, n * 4) != cudaSuccess)
+  h->poolMem = std::move(A);
+  for(int l = 0; l < h->numLanes; l++)
   {
-    cudaGetLastError();
-    h->dSelect = nullptr;
-    h->err = "selection image: out of device memory";
-    return fail(B200PT_E_NOMEM);
+    h->lanes[l].P = P[l];
+    std::copy(dQ[l], dQ[l] + 6, h->lanes[l].dQ);
   }
-  h->poolAllocs.push_back(h->dSelect);
-  if(cudaMalloc((void**)&h->dNdcDepth, n * 4) != cudaSuccess)
-  {
-    cudaGetLastError();
-    h->dNdcDepth = nullptr;
-    h->err = "depth image: out of device memory";
-    return fail(B200PT_E_NOMEM);
-  }
-  h->poolAllocs.push_back(h->dNdcDepth);
-  if(h->guides)
-  {
-    if(cudaMalloc((void**)&h->dGuide, n * 16) != cudaSuccess)
-    {
-      cudaGetLastError();
-      h->dGuide = nullptr;
-      h->err = "guide image: out of device memory";
-      return fail(B200PT_E_NOMEM);
-    }
-    h->poolAllocs.push_back(h->dGuide);
-    if(cudaMemsetAsync(h->dGuide, 0, n * 16, h->stream) != cudaSuccess)
-      return fail(B200PT_E_CUDA);
-  }
-  if(h->dlss)
-  {
-    if(cudaMalloc((void**)&h->dDlss, n * kDlssBytesPerPixel + 6 * 256) != cudaSuccess)
-    {
-      cudaGetLastError();
-      h->dDlss = nullptr;
-      h->err = "DLSS guide images: out of device memory";
-      return fail(B200PT_E_NOMEM);
-    }
-    h->poolAllocs.push_back(h->dDlss);
-    if(cudaMemsetAsync(h->dDlss, 0, n * kDlssBytesPerPixel + 6 * 256, h->stream) != cudaSuccess)
-      return fail(B200PT_E_CUDA);
-  }
-  if(cudaMalloc((void**)&h->dTonemapped, n * 4) != cudaSuccess)
-  {
-    cudaGetLastError();
-    h->dTonemapped = nullptr;
-    h->err = "tonemapped image: out of device memory";
-    return fail(B200PT_E_NOMEM);
-  }
-  h->poolAllocs.push_back(h->dTonemapped);
-  if(cudaMemsetAsync(h->dSelect, 0, n * 4, h->stream) != cudaSuccess || cudaMemsetAsync(h->dNdcDepth, 0, n * 4, h->stream) != cudaSuccess
-     || cudaMemsetAsync(h->dAccumOwned, 0, n * 16, h->stream) != cudaSuccess || cudaStreamSynchronize(h->stream) != cudaSuccess)
-  {
-    h->err = "b200pt_resize: clearing the accumulation image failed";
-    return fail(B200PT_E_CUDA);
-  }
+  h->dAccumOwned = accum;
+  h->dSelect = select;
+  h->dNdcDepth = ndcDepth;
+  h->dGuide = guide;
+  h->dDlss = dlss;
+  h->dTonemapped = tonemapped;
   h->width = width;
   h->height = height;
   h->tileY0 = tile_y0;
@@ -4091,11 +3982,8 @@ int b200pt_set_accum_device(b200pt_t* h, float* dev, size_t num_floats)
     h->dAccum = h->dAccumOwned;
     return B200PT_OK;
   }
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   if(num_floats < (size_t)h->numPaths * 4)
   {
     h->err = "b200pt_set_accum_device: buffer too small";
@@ -4120,12 +4008,8 @@ int b200pt_read_accum(b200pt_t* h, float* host, size_t num_floats)
 {
   if(!h || h->numPaths == 0 || !host || num_floats < (size_t)h->numPaths * 4)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   CK(cudaMemcpyAsync(host, h->dAccum, (size_t)h->numPaths * 16, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return B200PT_OK;
@@ -4169,12 +4053,8 @@ int b200pt_tonemap(b200pt_t* h, const b200pt_tonemapper* tm, uint8_t* host_rgba8
     h->err = "b200pt_tonemap: an interleaved multi-GPU tile is tonemapped after the gather (b200pt_tonemap_image on the full image)";
     return B200PT_E_UNSUPPORTED;
   }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   const int rc = tonemapOnDevice(h, tm, h->dAccum, h->width, h->tileRows, h->tileY0, h->height, h->dTonemapped, exposure_used);
   if(rc)
     return rc;
@@ -4208,12 +4088,8 @@ int b200pt_read_selection(b200pt_t* h, uint32_t* host_object_ids, float* host_nd
 {
   if(!h || h->numPaths == 0 || num_pixels < (size_t)h->numPaths || (!host_object_ids && !host_ndc_depth))
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   if(host_object_ids)
     CK(cudaMemcpyAsync(host_object_ids, h->dSelect, (size_t)h->numPaths * 4, cudaMemcpyDeviceToHost, h->stream));
   if(host_ndc_depth)
@@ -4237,12 +4113,8 @@ int b200pt_read_accum_async(b200pt_t* h, float* host, size_t num_floats, int slo
 {
   if(!h || h->numPaths == 0 || !host || num_floats < (size_t)h->numPaths * 4 || slot < 0 || slot >= 8)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   if(!h->readDone[slot])
     CK(cudaEventCreateWithFlags(&h->readDone[slot], cudaEventDisableTiming));
   else
@@ -4261,6 +4133,23 @@ int b200pt_wait_read(b200pt_t* h, int slot)
   return B200PT_OK;
 }
 
+// the path pool rebuilt at the current extent (interleaved or not) after a change of what it holds; an accumulation buffer the
+// caller supplied (b200pt_set_accum_device) stays in use
+static int rebuildPool(b200pt_t* h)
+{
+  if(h->numPaths == 0)
+    return B200PT_OK;
+  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
+  int           rc;
+  if(h->bandWorld > 1)
+    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
+  else
+    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
+  if(rc == B200PT_OK && user)
+    h->dAccum = user;
+  return rc;
+}
+
 int b200pt_set_frames_in_flight(b200pt_t* h, int n)
 {
   if(!h || n < 1 || n > b200pt::kMaxLanes)
@@ -4268,55 +4157,27 @@ int b200pt_set_frames_in_flight(b200pt_t* h, int n)
   if(n == h->numLanes)
     return B200PT_OK;
   h->numLanes = n;
-  if(h->numPaths == 0)
-    return B200PT_OK;
-  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
-  int           rc;
-  if(h->bandWorld > 1)
-    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
-  else
-    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
-  if(rc == B200PT_OK && user)
-    h->dAccum = user;
-  return rc;
+  return rebuildPool(h);
 }
 
 int b200pt_set_guide_outputs(b200pt_t* h, int enable)
 {
   if(!h)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   if((enable != 0) == h->guides)
     return B200PT_OK;
   h->guides = enable != 0;
-  if(h->numPaths == 0)
-    return B200PT_OK;
-  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
-  int           rc;
-  if(h->bandWorld > 1)
-    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
-  else
-    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
-  if(rc == B200PT_OK && user)
-    h->dAccum = user;
-  return rc;
+  return rebuildPool(h);
 }
 
 int b200pt_read_guide(b200pt_t* h, float* host_albedo_normal, size_t num_floats)
 {
   if(!h || h->numPaths == 0 || !h->dGuide || !host_albedo_normal || num_floats < (size_t)h->numPaths * 4)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   CK(cudaMemcpyAsync(host_albedo_normal, h->dGuide, (size_t)h->numPaths * 16, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   return B200PT_OK;
@@ -4336,26 +4197,12 @@ int b200pt_set_dlss_guides(b200pt_t* h, int enable)
 {
   if(!h)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   if((enable != 0) == h->dlss)
     return B200PT_OK;
   h->dlss = enable != 0;
-  if(h->numPaths == 0)
-    return B200PT_OK;
-  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
-  int           rc;
-  if(h->bandWorld > 1)
-    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
-  else
-    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
-  if(rc == B200PT_OK && user)
-    h->dAccum = user;
-  return rc;
+  return rebuildPool(h);
 }
 
 // the six planes inside dDlss, in the order of b200pt_dlss_guides; each starts on a 256-byte boundary (dlssAllocBytes)
@@ -4387,12 +4234,8 @@ int b200pt_read_dlss_guides(b200pt_t* h, const b200pt_dlss_guides* out)
       h->err = "b200pt_read_dlss_guides: a destination is smaller than its plane (tile_rows x width in the plane's format)";
       return B200PT_E_INVALID;
     }
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   for(int k = 0; k < 6; k++)
     if(host[k])
       CK(cudaMemcpyAsync(host[k], dev[k], need[k], cudaMemcpyDeviceToHost, h->stream));
@@ -4428,36 +4271,18 @@ int b200pt_set_frame_batch(b200pt_t* h, int n)
     return B200PT_E_INVALID;
   if(n == h->batch)
     return B200PT_OK;
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   h->batch = n;
-  if(h->numPaths == 0)
-    return B200PT_OK;
-  float4* const user = (h->dAccum != h->dAccumOwned) ? h->dAccum : nullptr;
-  int           rc;
-  if(h->bandWorld > 1)
-    rc = b200pt_resize_interleaved(h, h->width, h->height, h->bandRows, h->bandWorld, h->bandRank);
-  else
-    rc = b200pt_resize(h, h->width, h->height, h->tileY0, h->tileRows);
-  if(rc == B200PT_OK && user)
-    h->dAccum = user;
-  return rc;
+  return rebuildPool(h);
 }
 
 int b200pt_synchronize(b200pt_t* h)
 {
   if(!h)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   return checkDeviceErrors(h);
 }
 
@@ -4465,12 +4290,8 @@ int b200pt_set_profiling(b200pt_t* h, int enabled)
 {
   if(!h)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
+  if(const int rc = enter(h, false))
+    return rc;
   flushEvents(h);
   h->profiling = enabled != 0;
   if(h->profiling && h->evPool.empty())
@@ -4801,13 +4622,8 @@ int b200pt_get_stats(b200pt_t* h, b200pt_stats* out)
 {
   if(!h || !out)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   DevStats d{};
   CK(cudaMemcpy(&d, h->dStats, sizeof(d), cudaMemcpyDeviceToHost));
   out->closestRays = d.closestRays;
@@ -4842,13 +4658,8 @@ int b200pt_reset_stats(b200pt_t* h)
 {
   if(!h)
     return B200PT_E_INVALID;
-  CK(cudaSetDevice(h->device));
-  {
-    const int frc = flushPending(h);
-    if(frc)
-      return frc;
-  }
-  syncAll(h);
+  if(const int rc = enter(h, true))
+    return rc;
   CK(cudaMemset(h->dStats, 0, sizeof(DevStats)));
   flushEvents(h);
   for(int k = 0; k < 6; k++)
@@ -4868,28 +4679,17 @@ static int ensureRayPool(b200pt_t* h, uint32_t n)
     return B200PT_OK;
   syncAll(h);
   freeRayPool(h);
-  int rc = allocPathState(h, h->rayAllocs, n, h->rayP);
-  for(int k = 0; k < 3 && !rc; k++)
-  {
-    if(cudaMalloc((void**)&h->rayQ[k], (size_t)n * sizeof(uint32_t)) != cudaSuccess)
-      rc = B200PT_E_NOMEM;
-    else
-      h->rayAllocs.push_back(h->rayQ[k]);
-  }
-  if(!rc)
-  {
-    if(cudaMalloc((void**)&h->rayCounters, 8 * sizeof(uint32_t)) != cudaSuccess)
-      rc = B200PT_E_NOMEM;
-    else
-      h->rayAllocs.push_back(h->rayCounters);
-  }
-  if(rc)
-  {
-    cudaGetLastError();
-    freeRayPool(h);
-    h->err = "ray-level API: out of device memory";
-    return rc;
-  }
+  DeviceArena A;
+  PathState   P;
+  allocPathState(h, A, n, P);
+  uint32_t* const q[3] = {A.alloc<uint32_t>(n), A.alloc<uint32_t>(n), A.alloc<uint32_t>(n)};
+  uint32_t* const counters = A.alloc<uint32_t>(8);
+  if(!A.ok())
+    return failed(h, A, "ray-level API");
+  h->rayMem = std::move(A);
+  h->rayP = P;
+  std::copy(q, q + 3, h->rayQ);
+  h->rayCounters = counters;
   h->rayCapacity = n;
   return B200PT_OK;
 }

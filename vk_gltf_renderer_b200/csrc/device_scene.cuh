@@ -4,7 +4,7 @@
 // (shaders/gltf_scene_io.h.slang:41-322; shaders/shaderio.h:148-196), re-laid for CUDA:
 //   GltfRenderNode[] / GltfShadeMaterial[] / GltfTextureInfo[] / GltfLight[]  : same bytes, AoS
 //   GltfRenderPrimitive (7 device addresses)                                  : DevPrim
-//   bindless Sampler2D allTextures[]                                          : cudaTextureObject_t[]
+//   bindless Sampler2D allTextures[]                                          : DevTex[] (tiled mip chains in global memory)
 //   HDR env Sampler2D + StructuredBuffer<EnvAccel>                            : float4[] + uint2[]
 //   TLAS/BLAS                                                                 : BvhView (+ triMeta)
 #pragma once
