@@ -36,9 +36,7 @@ def lib():
         L.oracle_set_opacity_micromaps.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         L.oracle_set_environment.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]
         L.oracle_get_environment.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.oracle_render_frame.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.oracle_render_frame_aux.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
-        L.oracle_render_frame_guide.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
+        L.oracle_render_frame.argtypes = [C.c_void_p] * 9 + [C.c_int] * 3
         L.oracle_trace_closest.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
         L.oracle_trace_shadow.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
         L.oracle_trace_closest_mt.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_int]
@@ -46,6 +44,8 @@ def lib():
         L.oracle_bsdf_sample.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.oracle_bsdf_sample_simple.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.oracle_bsdf_eval_simple.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_dlss_env_brdf_approx2.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_dlss_motion_vector.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.oracle_get_stats.argtypes = [C.c_void_p, C.c_void_p]
         L.oracle_reset_stats.argtypes = [C.c_void_p]
         L.oracle_num_tris.argtypes = [C.c_void_p]
@@ -65,6 +65,10 @@ def _p(a):
 
 
 class Oracle:
+    # the DLSS guide planes (name, dtype, channels), in the order of oracle_render_frame's dlssPlanes
+    DLSS_PLANES = (("albedo", np.uint8, 4), ("spec_albedo", np.float16, 4), ("normal_roughness", np.float16, 4),
+                   ("motion", np.float16, 2), ("depth", np.float16, 1), ("spec_hit_dist", np.float16, 1))
+
     def __init__(self):
         self.L = lib()
         self.h = C.c_void_p(self.L.oracle_create())
@@ -111,10 +115,32 @@ class Oracle:
     def render_frame(self, fi, pc, accum, y0=0, rows=None, threads=None, object_id=None, ndc_depth=None, guide=None):
         """accum: float32 [rows, W, 4], updated in place (running mean like processPixel).  object_id (uint32 [rows, W]) /
         ndc_depth (float32 [rows, W]), if given, receive the frame-0 outputs (selection ray id, NDC depth of the first hit);
-        guide (float32 [rows, W, 4]) the eOptixAlbedoNormal image of a frame whose push constants carry ePtUseOptixDenoiser."""
+        guide (float32 [rows, W, 4]) the eOptixAlbedoNormal image of a frame whose push constants carry ePtUseOptixDenoiser.
+        A DLSS frame (pc carries PT_USE_DLSS) raises ValueError: it writes guide planes, so it goes through render_frame_dlss."""
+        self._render_frame(fi, pc, accum, y0, rows, threads, object_id, ndc_depth, guide)
+
+    def render_frame_dlss(self, fi, pc, accum, prev_object_to_world=None, y0=0, rows=None, threads=None, object_id=None, ndc_depth=None,
+                          guide=None):
+        """A frame of the DLSS variant (pc carries PT_USE_DLSS): accum (float32 [rows, W, 4]) is replaced; returns the six guide
+        planes as a dict of arrays shaped like PathTracer.read_dlss_guides().  prev_object_to_world: float32 [numRenderNodes, 16]
+        (the previous frame's objectToWorld, glm order) or None for camera-only motion.  A frame the variant refuses (no PT_USE_DLSS,
+        numSamples != 1) raises ValueError."""
+        rows = accum.shape[0] if rows is None else rows
+        w = accum.shape[1]
+        planes = {name: np.zeros((rows, w, ch) if ch > 1 else (rows, w), dt) for name, dt, ch in self.DLSS_PLANES}
+        prev = None if prev_object_to_world is None else np.ascontiguousarray(prev_object_to_world, np.float32)
+        self._render_frame(fi, pc, accum, y0, rows, threads, object_id, ndc_depth, guide, prev, planes)
+        return planes
+
+    def _render_frame(self, fi, pc, accum, y0, rows, threads, object_id, ndc_depth, guide, prev=None, planes=None):
         rows = accum.shape[0] if rows is None else rows
         threads = threads or os.cpu_count() or 1
-        rc = self.L.oracle_render_frame_guide(self.h, C.byref(fi), C.byref(pc), _p(accum), _p(object_id), _p(ndc_depth), _p(guide), y0, rows, threads)
+        ptrs = None if planes is None else (C.c_void_p * 6)(*[planes[name].ctypes.data for name, _, _ in self.DLSS_PLANES])
+        rc = self.L.oracle_render_frame(self.h, C.byref(fi), C.byref(pc), _p(accum), _p(object_id), _p(ndc_depth), _p(guide), _p(prev), ptrs,
+                                        y0, rows, threads)
+        if rc == -1:   # B200PT_E_INVALID
+            raise ValueError("oracle_render_frame: a DLSS frame (PT_USE_DLSS) needs numSamples == 1 and the guide planes of render_frame_dlss; "
+                             "a plain frame takes no planes")
         if rc:
             raise RuntimeError(f"oracle_render_frame failed: {rc}")
 
@@ -182,6 +208,21 @@ class Oracle:
         out = np.empty((len(records), 4), np.float32)
         if self.L.oracle_texture_lookup(self.h, _p(records), len(records), _p(out)):
             raise ValueError("oracle_texture_lookup: a record has a texture-info slot outside the scene or a mode other than 0 / 1")
+        return out
+
+    def env_brdf_approx2(self, records):
+        """EnvBRDFApprox2 on float32 [n, 5] records (specular colour xyz, alpha, NoV) -> [n, 3]"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 5)
+        out = np.empty((len(records), 3), np.float32)
+        self.L.oracle_dlss_env_brdf_approx2(_p(records), len(records), _p(out))
+        return out
+
+    def motion_vector(self, records, prev_mvp, curr_mvp):
+        """calculateMotionVector on float32 [n, 10] records (current xyzw, previous xyzw, resolution xy) -> pixel motion [n, 2]"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 10)
+        out = np.empty((len(records), 2), np.float32)
+        self.L.oracle_dlss_motion_vector(_p(records), len(records), _p(np.ascontiguousarray(prev_mvp, np.float32)),
+                                    _p(np.ascontiguousarray(curr_mvp, np.float32)), _p(out))
         return out
 
 

@@ -13,6 +13,9 @@
 //   evaluateMaterial / getTexture                                   shaders/gltf_material_eval.h.slang:76-457
 //   getOpacity / getShadowTransmission                              shaders/pathtrace_functions.h.slang:189-343
 //   instance flags (opaque / cull-disable)                          src/gltf_scene_rtx.cpp:271-295
+//   DLSS variant: jitter, captures, guide images                    shaders/gltf_pathtrace.slang:135-143, 216-263, 370-377, 564-651,
+//                                                                   shaders/pathtrace_functions.h.slang:65-102, 942-988
+//   EnvBRDFApprox2 / calculateMotionVector                          shaders/dlss_util.h
 // and, in bsdf.h, the EXTERNAL nvpro_core2/nvshaders arithmetic (BSDF, RNG, env sampling ...).
 //
 // PARITY UNPINNED.  The reference cannot be built or run here (needs Vulkan-RT, slangc,
@@ -35,6 +38,7 @@
 #include <cfloat>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <thread>
 #include <vector>
 
@@ -1464,6 +1468,8 @@ struct Ctx
   Oracle*                     o;
   const b200pt_frame_info*    fi;
   const b200pt_push_constant* pc;
+  bool                        dlss;               // a DLSS frame (pc carries B200PT_PT_USE_DLSS): the USE_DLSS_SHADER captures
+  const float*                prevObjectToWorld;  // DLSS: previous-frame objectToWorld per render node (16 floats, glm order), or null: camera-only motion
 };
 
 struct DirectLight
@@ -1595,10 +1601,76 @@ static bool hasVolumeMedium(const VolumeMedium& v) { return maxc(v.extinction) >
 // value of x after a round trip through IEEE binary16 (round to nearest even): the reference's float16_t guide fields
 static inline float half16(float x) { return (float)(_Float16)x; }
 
+static inline uint16_t halfBits(float x)
+{
+  const _Float16 h = (_Float16)x;
+  uint16_t       b;
+  memcpy(&b, &h, 2);
+  return b;
+}
+static uint32_t unorm8(float x) { return (uint32_t)roundf(fminf(fmaxf(x, 0.0f), 1.0f) * 255.0f); }
+
+// ---- DLSS guide arithmetic (shaders/dlss_util.h), restated: Slang matrices are row-major, mul(M, v)[r] = dot(row r, v), dot and
+//      mul sum left to right, rcp(x) = 1 / x, mad(a, b, c) = a * b + c (unfused, like the rest of the oracle)
+template <int N>
+static float dotN(const float* a, const float* b)
+{
+  float r = a[0] * b[0];
+  for(int k = 1; k < N; k++)
+    r = r + a[k] * b[k];
+  return r;
+}
+template <int N>
+static void mulMv(const float (&M)[N][N], const float* v, float* out)
+{
+  for(int r = 0; r < N; r++)
+    out[r] = dotN<N>(M[r], v);
+}
+
+// EnvBRDFApprox2(SpecularColor, alpha, NoV): Ray Tracing Gems chapter 32 fit of the split-sum specular albedo
+static float3 envBRDFApprox2(float3 specularColor, float alpha, float NoV)
+{
+  NoV = fabsf(NoV);
+  const float X[4] = {1.0f, NoV, NoV * NoV, NoV * (NoV * NoV)};
+  const float Y[4] = {1.0f, alpha, alpha * alpha, alpha * (alpha * alpha)};
+  static const float M1[2][2] = {{0.99044f, -1.28514f}, {1.29678f, -0.755907f}};
+  static const float M2[3][3] = {{1.f, 2.92338f, 59.4188f}, {20.3225f, -27.0302f, 222.592f}, {121.563f, 626.13f, 316.627f}};
+  static const float M3[2][2] = {{0.0365463f, (float)3.32707}, {9.0632f, (float)-9.04756}};
+  static const float M4[3][3] = {{1.f, 3.59685f, -1.36772f}, {9.04401f, -16.3174f, 9.22949f}, {5.56589f, 19.7886f, -20.2123f}};
+  const float xy[2] = {X[0], X[1]}, xyw[3] = {X[0], X[1], X[3]}, xzw[3] = {X[0], X[2], X[3]};
+  const float yxy[2] = {Y[0], Y[1]}, yxyw[3] = {Y[0], Y[1], Y[3]};
+  float       a[3], b[3];
+  mulMv(M1, xy, a);
+  mulMv(M2, xyw, b);
+  float bias = dotN<2>(a, yxy) * (1.0f / dotN<3>(b, yxyw));
+  mulMv(M3, xy, a);
+  mulMv(M4, xzw, b);
+  const float scale = dotN<2>(a, yxy) * (1.0f / dotN<3>(b, yxyw));
+  bias *= fminf(fmaxf(specularColor.y * 50.0f, 0.0f), 1.0f);
+  const float sc = fmaxf(0.0f, scale), bi = fmaxf(0.0f, bias);
+  return f3(specularColor.x * sc + bi, specularColor.y * sc + bi, specularColor.z * sc + bi);
+}
+
+// calculateMotionVector(currWorldPos, prevWorldPos, prevMVP, currentMVP, resolution): mul(float4, float4x4) on the glm bytes
+static float2 calculateMotionVector(float4 currWorld, float4 prevWorld, const mat4& prevMVP, const mat4& currMVP, float2 resolution)
+{
+  const float4 currClip = mul_vM(currWorld, currMVP);
+  const float4 prevClip = mul_vM(prevWorld, prevMVP);
+  const float2 currNDC = f2(currClip.x / currClip.w, currClip.y / currClip.w);
+  const float2 prevNDC = f2(prevClip.x / prevClip.w, prevClip.y / prevClip.w);
+  return f2((prevNDC.x - currNDC.x) * 0.5f * resolution.x, (prevNDC.y - currNDC.y) * 0.5f * resolution.y);
+}
+
 struct PathTracerState
 {
   float3       radiance = f3(0.0f), throughput = f3(1.0f), firstHitPos = f3(1e34f);
   float3       guideAlbedo = f3(0.0f), guideNormal = f3(0.0f);  // GuideScratch (pathtrace_functions.h.slang:79-88): float16_t fields, default 0
+  // USE_DLSS_SHADER: the rest of GuideScratch and the first hit's previous-frame position, written on DLSS frames only
+  float        guideRoughness = 0.0f;
+  float3       firstHitPosPrev = f3(1e34f);
+  float3       specAlbedo = f3(0.0f);  // GuideScratch::specularAlbedo (float16_t)
+  float        specHitDist = 0.0f;     // GuideScratch::specularHitDist (float16_t)
+  bool         captureSpecularHit = false;
   float        lastSamplePdf = DIRAC;
   float2       maxRoughness = f2(0.0f, 0.0f);
   bool         solid = true;
@@ -1693,8 +1765,32 @@ static PathStepResult processVolumeSegment(const Ctx& c, float hitDistance, Ray&
   return eOutOfVolume;
 }
 
-// pathTraceOneBounce (gltf_pathtrace.slang:87-430); infinite plane / backplate blur / DLSS / viz paths
-// are off in every BASELINE config and are not restated.
+// The DLSS guides of the first hit (gltf_pathtrace.slang:235-255): roughness, previous-frame position and specular albedo.  node is
+// the hit's render node, null for the infinite plane.  Kept out of line so that the bounce stays small enough for GCC to inline
+// evaluateMaterial into it, as it does without the DLSS captures: plain frames then run the code they ran before the variant.
+__attribute__((noinline)) static void dlssFirstHitGuides(const Ctx& c, const PbrMaterial& pbrMat, float3 pos, const b200pt_render_node* node, int rnodeID,
+                                                         float3 rayDir, PathTracerState& pt)
+{
+  pt.guideRoughness = half16(pbrMat.roughness.x);
+  // instance motion (:235-241): the surface point in object space, then through the previous frame's objectToWorld
+  pt.firstHitPosPrev = pos;
+  if(node && c.prevObjectToWorld)
+  {
+    const float4 objPos = mul_vM(f4(pos.x, pos.y, pos.z, 1.0f), *(const mat4*)node->worldToObject);
+    pt.firstHitPosPrev = xyz(mul_vM(f4(objPos.x, objPos.y, objPos.z, 1.0f), *(const mat4*)(c.prevObjectToWorld + 16 * (size_t)rnodeID)));
+  }
+  // specular albedo (:246-255); pow(x, 2.0) is the correctly rounded square
+  const float  q = (pbrMat.ior2 - pbrMat.ior1) / (pbrMat.ior2 + pbrMat.ior1);
+  const float  f0FromIor = q * q;
+  const float3 clamped = f3(fminf(f0FromIor * pbrMat.specularColor.x, 1.0f), fminf(f0FromIor * pbrMat.specularColor.y, 1.0f),
+                            fminf(f0FromIor * pbrMat.specularColor.z, 1.0f));
+  const float3 sa = envBRDFApprox2(clamped, pbrMat.roughness.x, dot(pbrMat.N, rayDir));
+  pt.specAlbedo = f3(half16(sa.x), half16(sa.y), half16(sa.z));
+}
+
+// pathTraceOneBounce (gltf_pathtrace.slang:87-430) with the infinite plane, the shadow catcher and, on DLSS frames, the
+// USE_DLSS_SHADER captures (the reference's shader specialization: a plain frame arms no capture and computes no DLSS guide).
+// The backplate blur is refused by the frame entry; the visualization modes are not restated.
 static PathStepResult pathTraceOneBounce(const Ctx& c, Ray& ray, uint32_t& seed, PathTracerState& pt, BounceScratch& bounce)
 {
   Oracle& o = *c.o;
@@ -1745,11 +1841,18 @@ static PathStepResult pathTraceOneBounce(const Ctx& c, Ray& ray, uint32_t& seed,
       // tryPrimaryMissBackplate (pathtrace_functions.h.slang:944-971)
       pt.solid = false;
       pt.firstHitPos = ray.d;
+      pt.firstHitPosPrev = ray.d;
       if(c.fi->flags & B200PT_SCENE_USE_SOLID_BACKGROUND)
       {
         pt.radiance = f3(c.fi->backgroundColor[0], c.fi->backgroundColor[1], c.fi->backgroundColor[2]);
         return eBreak;
       }
+    }
+    // DLSS: a glossy reflection of the first hit leaves to the sky (gltf_pathtrace.slang:135-143)
+    if(pt.captureSpecularHit)
+    {
+      pt.specHitDist = 65504.0f;
+      pt.captureSpecularHit = false;
     }
     float3 envColor;
     float  envPdf;
@@ -1858,13 +1961,22 @@ static PathStepResult pathTraceOneBounce(const Ctx& c, Ray& ray, uint32_t& seed,
     pbrMat = evaluateMaterial(o, o.mats[materialIndex], mesh);
   }
 
+  // DLSS: the first surface behind a glossy reflection of the first hit (:216-223); the shadow catcher returned above
+  if(pt.captureSpecularHit)
+  {
+    pt.specHitDist = half16(payload.hitT);
+    pt.captureSpecularHit = false;
+  }
+
   if(firstRay)
   {
     pt.firstHitPos = hit.pos;
-    // USE_GUIDE_SHADER (gltf_pathtrace.slang:240-263, without the DLSS-only specular guides): base colour and shading normal of
-    // the first hit, stored as float16_t by the reference
+    // USE_GUIDE_SHADER (gltf_pathtrace.slang:240-263): base colour, shading normal and, on DLSS frames, roughness of the first hit,
+    // stored as float16_t by the reference
     pt.guideAlbedo = f3(half16(pbrMat.baseColor.x), half16(pbrMat.baseColor.y), half16(pbrMat.baseColor.z));
     pt.guideNormal = f3(half16(pbrMat.N.x), half16(pbrMat.N.y), half16(pbrMat.N.z));
+    if(c.dlss)
+      dlssFirstHitGuides(c, pbrMat, hit.pos, hitInfinitePlane ? nullptr : &o.nodes[payload.rnodeID], payload.rnodeID, ray.d, pt);
   }
 
   pt.maxRoughness = f2(fmaxf(pbrMat.roughness.x, pt.maxRoughness.x), fmaxf(pbrMat.roughness.y, pt.maxRoughness.y));
@@ -1923,6 +2035,9 @@ static PathStepResult pathTraceOneBounce(const Ctx& c, Ray& ray, uint32_t& seed,
     pt.throughput *= sd.bsdf_over_pdf;
     ray.d = sd.k2;
     pt.lastSamplePdf = sd.pdf;
+    // DLSS: arm the specular hit-distance capture (:370-377)
+    if(c.dlss && firstRay && (sd.event_type == BSDF_EVENT_GLOSSY_REFLECTION || sd.event_type == BSDF_EVENT_IMPULSE_REFLECTION))
+      pt.captureSpecularHit = true;
     if(sd.event_type != BSDF_EVENT_ABSORB)
     {
       bool   isTransmission = (sd.event_type & BSDF_EVENT_TRANSMISSION) != 0;
@@ -1953,6 +2068,9 @@ struct SampleResult
   float4 radiance;
   float3 hitPosition;
   float3 guideAlbedo, guideNormal;  // SampleResult::guideOutput (pathtrace_functions.h.slang:94-102)
+  float  guideRoughness;            // DLSS frames: the rest of guideOutput and the first hit's previous-frame position
+  float3 hitPositionPrev, specAlbedo;
+  float  specHitDist;
 };
 
 static SampleResult pathTrace(const Ctx& c, Ray ray, uint32_t& seed)
@@ -1995,6 +2113,10 @@ static SampleResult pathTrace(const Ctx& c, Ray ray, uint32_t& seed)
   r.hitPosition = pt.firstHitPos;
   r.guideAlbedo = pt.guideAlbedo;
   r.guideNormal = pt.guideNormal;
+  r.guideRoughness = pt.guideRoughness;
+  r.hitPositionPrev = pt.firstHitPosPrev;
+  r.specAlbedo = pt.specAlbedo;
+  r.specHitDist = pt.specHitDist;
   return r;
 }
 
@@ -2051,7 +2173,6 @@ static float2 sampleGaussian(float2 u)
   return f2(r * cosf(theta), r * sinf(theta));
 }
 
-// processPixel (gltf_pathtrace.slang:546-630); accum is the tile's RGBA32F image
 // TraceLow (raytracer_interface.h.slang:124-137): every triangle opaque, no culling -> nearest hit of both trees
 static int traceLowObjectId(Oracle& o, const Ray& ray)
 {
@@ -2082,7 +2203,20 @@ static uint32_t compressUnitVec(float3 nv)
   return packed == ~0u ? ~1u : packed;
 }
 
-static void processPixel(const Ctx& c, int x, int y, float* px, uint32_t* objectId = nullptr, float* ndcDepth = nullptr, float* guide = nullptr)
+// the DLSS guide planes of one pixel
+struct DlssOut
+{
+  uint32_t* albedo;       // RGBA8 UNORM
+  uint16_t* specAlbedo;   // RGBA16F
+  uint16_t* normalRough;  // RGBA16F
+  uint16_t* motion;       // RG16F
+  uint16_t* depth;        // R16F
+  uint16_t* specHitDist;  // R16F
+};
+
+// processPixel (gltf_pathtrace.slang:546-651).  A DLSS frame (dlss non-null, numSamples == 1) samples at the frame's jitter, replaces
+// the image and writes the guide planes.
+static void processPixel(const Ctx& c, int x, int y, float* px, uint32_t* objectId, float* ndcDepth, float* guide, const DlssOut* dlss)
 {
   const float2 imageSize = f2(c.fi->imageSize[0], c.fi->imageSize[1]);
   const float2 samplePos = f2((float)x, (float)y);
@@ -2090,6 +2224,9 @@ static void processPixel(const Ctx& c, int x, int y, float* px, uint32_t* object
   dbgPixel = ((float)x == c.pc->mouseCoord[0] && (float)y == c.pc->mouseCoord[1]);
   const bool   firstFrame = (c.pc->flags & B200PT_PT_FIRST_FRAME) != 0;
   float2       jitter = f2(0.5f, 0.5f);
+  if(c.dlss)
+    jitter = f2(0.5f + c.fi->jitter[0], 0.5f + c.fi->jitter[1]);  // the frame's DLSS jitter; no Gaussian draw (gltf_pathtrace.slang:568-572)
+  else
   {
     float  a = rnd(seed), b = rnd(seed);
     float2 g = sampleGaussian(f2(a, b));
@@ -2143,7 +2280,33 @@ static void processPixel(const Ctx& c, int x, int y, float* px, uint32_t* object
     guide[2] = sr.guideAlbedo.z;
     memcpy(&guide[3], &packed, 4);
   }
-  if(firstFrame)
+  if(dlss)
+  {
+    // gltf_pathtrace.slang:628-651
+    const bool   hasSolidHit = sr.radiance.w > 0.0f;
+    float        d = 1.0f;
+    const mat4&  vp = *(const mat4*)c.fi->viewProjMatrix;
+    if(hasSolidHit)
+    {
+      const float4 clip = mul_vM(f4(sr.hitPosition.x, sr.hitPosition.y, sr.hitPosition.z, 1.0f), vp);
+      d = clip.z / clip.w;
+    }
+    const float  hitW = hasSolidHit ? 1.0f : 0.0f;
+    const float2 mv = calculateMotionVector(f4(sr.hitPosition.x, sr.hitPosition.y, sr.hitPosition.z, hitW),
+                                            f4(sr.hitPositionPrev.x, sr.hitPositionPrev.y, sr.hitPositionPrev.z, hitW), *(const mat4*)c.fi->prevMVP, vp, imageSize);
+    *dlss->depth = halfBits(d);
+    dlss->motion[0] = halfBits(mv.x);
+    dlss->motion[1] = halfBits(mv.y);
+    const float nr[4] = {sr.guideNormal.x, sr.guideNormal.y, sr.guideNormal.z, sr.guideRoughness};
+    for(int k = 0; k < 4; k++)
+      dlss->normalRough[k] = halfBits(nr[k]);
+    *dlss->albedo = unorm8(sr.guideAlbedo.x) | (unorm8(sr.guideAlbedo.y) << 8) | (unorm8(sr.guideAlbedo.z) << 16) | (unorm8(hitW) << 24);
+    const float sa[4] = {sr.specAlbedo.x, sr.specAlbedo.y, sr.specAlbedo.z, 1.0f};
+    for(int k = 0; k < 4; k++)
+      dlss->specAlbedo[k] = halfBits(sa[k]);
+    *dlss->specHitDist = halfBits(sr.specHitDist);
+  }
+  if(firstFrame || c.dlss)
   {
     px[0] = pixelColor.x;
     px[1] = pixelColor.y;
@@ -2323,33 +2486,28 @@ int oracle_get_environment(void* h, float* rgba, uint32_t* alias, float* q)
   return 0;
 }
 
-// renders rows [y0, y0+rows) of the frame into accum (rows x width x 4 floats, tile-local)
-int oracle_render_frame_aux(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, uint32_t* objectId, float* ndcDepth, int y0, int rows,
-                            int nthreads);
-int oracle_render_frame(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, int y0, int rows, int nthreads)
-{
-  return oracle_render_frame_aux(h, fi, pc, accum, nullptr, nullptr, y0, rows, nthreads);
-}
-
-int oracle_render_frame_guide(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, uint32_t* objectId, float* ndcDepth, float* guide,
-                              int y0, int rows, int nthreads);
-// objectId / ndcDepth (rows x width, tile-local, may be null): the frame-0 outputs of processPixel
-int oracle_render_frame_aux(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, uint32_t* objectId, float* ndcDepth, int y0, int rows,
-                            int nthreads)
-{
-  return oracle_render_frame_guide(h, fi, pc, accum, objectId, ndcDepth, nullptr, y0, rows, nthreads);
-}
-
-// guide (rows x width x 4 floats, may be null): OutputImage::eOptixAlbedoNormal, written when pc carries B200PT_PT_USE_OPTIX_DENOISER
-int oracle_render_frame_guide(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, uint32_t* objectId, float* ndcDepth, float* guide,
-                              int y0, int rows, int nthreads)
+// Renders rows [y0, y0+rows) of the frame into accum (rows x width x 4 floats, tile-local): the running mean of processPixel, or the
+// replaced image of a DLSS frame (pc carries B200PT_PT_USE_DLSS).  The other outputs are tile-local and may be null:
+//   objectId / ndcDepth (rows x width): the frame-0 outputs of processPixel;
+//   guide (rows x width x 4 floats): OutputImage::eOptixAlbedoNormal, written when pc carries B200PT_PT_USE_OPTIX_DENOISER;
+//   prevObjectToWorld: the previous frame's objectToWorld, 16 floats per render node, for a DLSS frame's instance motion; null gives
+//   camera-only motion;
+//   dlssPlanes: six pointers to the DLSS guide planes (rows x width each): albedo RGBA8, specular albedo RGBA16F, normal / roughness
+//   RGBA16F, motion RG16F, depth R16F, specular hit distance R16F.
+// Like b200pt_render_frame, B200PT_E_INVALID for a DLSS frame without the planes or with numSamples != 1, and for planes with a plain
+// frame.
+int oracle_render_frame(void* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, float* accum, uint32_t* objectId, float* ndcDepth, float* guide,
+                        const float* prevObjectToWorld, void* const* dlssPlanes, int y0, int rows, int nthreads)
 {
   Oracle& o = *(Oracle*)h;
   if(!(fi->flags & B200PT_SCENE_USE_HDR_ENVIRONMENT) || o.envW == 0)
     return B200PT_E_UNSUPPORTED;
   if(fi->envBlur > 0.0f && !(fi->flags & B200PT_SCENE_USE_SOLID_BACKGROUND))
     return B200PT_E_UNSUPPORTED;  // tryPrimaryMissBackplate's smoothHDRBlur (nvshaders, external)
-  Ctx       c{&o, fi, pc};
+  const bool dlss = (pc->flags & B200PT_PT_USE_DLSS) != 0;
+  if(dlss != (dlssPlanes != nullptr) || (dlss && pc->numSamples != 1))
+    return B200PT_E_INVALID;
+  const Ctx c{&o, fi, pc, dlss, prevObjectToWorld};
   const int W = (int)fi->imageSize[0];
   nthreads = std::max(1, nthreads);
   std::atomic<int>         next{0};
@@ -2361,8 +2519,14 @@ int oracle_render_frame_guide(void* h, const b200pt_frame_info* fi, const b200pt
       if(r >= rows)
         break;
       for(int x = 0; x < W; x++)
-        processPixel(c, x, y0 + r, accum + ((size_t)r * W + x) * 4, objectId ? objectId + (size_t)r * W + x : nullptr, ndcDepth ? ndcDepth + (size_t)r * W + x : nullptr,
-                     guide ? guide + ((size_t)r * W + x) * 4 : nullptr);
+      {
+        const size_t  p = (size_t)r * W + x;
+        const DlssOut d = dlss ? DlssOut{(uint32_t*)dlssPlanes[0] + p, (uint16_t*)dlssPlanes[1] + 4 * p, (uint16_t*)dlssPlanes[2] + 4 * p,
+                                         (uint16_t*)dlssPlanes[3] + 2 * p, (uint16_t*)dlssPlanes[4] + p, (uint16_t*)dlssPlanes[5] + p}
+                               : DlssOut{};
+        processPixel(c, x, y0 + r, accum + p * 4, objectId ? objectId + p : nullptr, ndcDepth ? ndcDepth + p : nullptr, guide ? guide + p * 4 : nullptr,
+                     dlss ? &d : nullptr);
+      }
     }
     o.stats.merge();
   };
@@ -2563,6 +2727,32 @@ int oracle_bsdf_sample_simple(const float* in, uint32_t n, float* out)
     q[5] = d.bsdf_over_pdf.z;
     q[6] = d.pdf;
     q[7] = (float)d.event_type;
+  }
+  return 0;
+}
+
+// DLSS arithmetic on records: EnvBRDFApprox2 on (specular colour xyz, alpha, NoV) -> rgb; calculateMotionVector on (current xyzw,
+// previous xyzw, resolution xy) with the two view-projection matrices (glm order) -> pixel motion xy
+int oracle_dlss_env_brdf_approx2(const float* in, uint32_t n, float* out)
+{
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float* p = in + 5 * (size_t)i;
+    const float3 r = envBRDFApprox2(f3(p[0], p[1], p[2]), p[3], p[4]);
+    out[3 * i + 0] = r.x;
+    out[3 * i + 1] = r.y;
+    out[3 * i + 2] = r.z;
+  }
+  return 0;
+}
+int oracle_dlss_motion_vector(const float* in, uint32_t n, const float* prevMVP, const float* currMVP, float* out)
+{
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float* p = in + 10 * (size_t)i;
+    const float2 mv = calculateMotionVector(f4(p[0], p[1], p[2], p[3]), f4(p[4], p[5], p[6], p[7]), *(const mat4*)prevMVP, *(const mat4*)currMVP, f2(p[8], p[9]));
+    out[2 * i + 0] = mv.x;
+    out[2 * i + 1] = mv.y;
   }
   return 0;
 }

@@ -1,6 +1,7 @@
 """The DLSS variant without a GPU: the host mirror's Halton jitter, the DEVICE arithmetic (csrc/dlss_guides.cuh) compiled for the
 host against the oracle's independent restatement and float64, and known answers of the oracle's six guide images on a synthetic
-scene (a camera-facing diffuse quad, a mirror facing a diffuse wall, open sky).  The oracle's DLSS variant is tests/dlss_oracle.cpp."""
+scene (a camera-facing diffuse quad, a mirror facing a diffuse wall, open sky).  The oracle restates the DLSS variant in
+oracle/pt_oracle.cpp, in the same bounce and pixel functions as the plain path tracer."""
 import math
 import os
 import subprocess
@@ -8,8 +9,6 @@ import sys
 
 import numpy as np
 import pytest
-
-from dlss_oracle import DlssOracle
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
@@ -90,7 +89,7 @@ def test_env_brdf_approx2_device_source_matches_oracle_and_float64(host_dlss, or
     rec[:8, 4] = [0, 0, 1, 1, -1, 1e-3, 0.5, -0.2]
     rec[8:12, :3] = 0.0                                  # specular reflectance 0: the bias hack
     dev = host_dlss("brdf", rec, np.float32).reshape(n, 3)
-    ref = DlssOracle().env_brdf_approx2(rec)
+    ref = oracle_mod.Oracle().env_brdf_approx2(rec)
     assert np.array_equal(dev.view(np.uint32), ref.view(np.uint32))
     exp = np.array([env_brdf64(r[:3], r[3], r[4]) for r in rec.astype(np.float64)])
     assert np.all(np.abs(ref - exp) <= 1e-5 * np.maximum(np.abs(exp), 1e-2))
@@ -113,7 +112,7 @@ def test_motion_vector_device_source_matches_oracle_and_float64(host_dlss, oracl
     moved = pts + rng.normal(0, 0.05, (n, 3)) * w[:, None]
     rec = np.concatenate([pts, w[:, None], moved, w[:, None], np.tile([64.0, 48.0], (n, 1))], 1).astype(np.float32)
     dev = host_dlss("motion", np.concatenate([prev, curr, rec.reshape(-1)]), np.float32).reshape(n, 2)
-    ref = DlssOracle().motion_vector(rec, prev, curr)
+    ref = oracle_mod.Oracle().motion_vector(rec, prev, curr)
     assert np.array_equal(dev.view(np.uint32), ref.view(np.uint32))
     for r, got in zip(rec.astype(np.float64), ref.astype(np.float64)):
         exp = motion64(r[0:4], r[4:8], prev.astype(np.float64), curr.astype(np.float64), r[8:10])
@@ -203,7 +202,7 @@ def project(p, vp):
 
 @pytest.fixture(scope="module")
 def kat(oracle_mod):
-    o = DlssOracle()
+    o = oracle_mod.Oracle()
     scn = kat_scene()
     o.set_scene(scn)
     o.set_environment(const_env())
@@ -258,7 +257,7 @@ def test_camera_translation_moves_surfaces_not_the_sky(kat):
 
 
 def test_instance_motion_follows_the_previous_transforms(oracle_mod):
-    o = DlssOracle()
+    o = oracle_mod.Oracle()
     before = kat_scene()
     o.set_environment(const_env())
     prev = np.stack([np.asarray(rn["objectToWorld"], np.float32) for rn in before.render_nodes])
@@ -337,3 +336,6 @@ def test_dlss_frame_refusals(kat):
     pc.flags &= ~abi.PT_USE_DLSS
     with pytest.raises(ValueError):
         o.render_frame_dlss(fi, pc, accum)   # a plain frame is not the DLSS variant
+    fi, pc = dlss_frame(scn.camera, 1)
+    with pytest.raises(ValueError):
+        o.render_frame(fi, pc, accum)        # a DLSS frame needs the guide planes

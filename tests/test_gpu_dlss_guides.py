@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 
 from conftest import rel_rmse
-from dlss_oracle import DlssOracle
 
 pytestmark = pytest.mark.gpu
 W, H = 128, 96
@@ -116,7 +115,7 @@ class Case:
 
     def run_oracle(self, oracle_mod, optix=False):
         from vk_gltf_renderer_b200 import abi, camera as camm
-        o = DlssOracle()
+        o = oracle_mod.Oracle()
         o.set_environment(self.env)
         o.set_scene(self.scn)
         s = self.settings
