@@ -19,3 +19,7 @@ for f in range(4):
         pt.set_profiling(True)
     pt.onRender(None, res)
 pt.synchronize()
+# the profiled frame's per-stage totals: each stage's column of the per-bounce rows above adds up to these
+st = pt.stats()
+print("frame totals:", "  ".join(f"{k} {st[k]:.3f}" for k in ("msTraceClosest", "msAnyHit", "msShade", "msTraceShadow", "msResolve", "msOther")) + " ms",
+      file=sys.stderr)

@@ -41,3 +41,32 @@ def random_rays(n, lo, hi, seed=1234):
     rays[:, 4:7] = d
     rays[:, 7] = 1e32
     return rays
+
+
+def trace_both(pt, o, rays, seeds, tmax=4.0, float_cols=()):
+    """Closest-hit rays, then the same rays as shadow rays cut at tmax, through the device's ray-level API and the oracle.
+    The hits must be equal bit for bit, except the columns in float_cols, which are compared as floats.  The seeds and the
+    shadow transmission must be exact.  Returns the oracle's hits, seeds, transmission and shadow-ray seeds."""
+    import torch
+    s_ref = seeds.copy()
+    ref = o.trace_closest(rays, s_ref)
+    d_rays, d_seeds = to_dev(rays), to_dev(seeds.copy())
+    d_hits = torch.empty((len(rays), 6), dtype=torch.float32, device="cuda")
+    pt.trace_closest(d_rays.data_ptr(), len(rays), d_hits.data_ptr(), d_seeds.data_ptr())
+    pt.synchronize()
+    got = d_hits.cpu().numpy()
+    bits = [c for c in range(got.shape[1]) if c not in float_cols]
+    assert np.array_equal(got.view(np.uint32)[:, bits], ref.view(np.uint32)[:, bits])
+    assert np.array_equal(got[:, list(float_cols)], ref[:, list(float_cols)])
+    assert np.array_equal(d_seeds.cpu().numpy(), s_ref)
+    rays_s = rays.copy()
+    rays_s[:, 7] = tmax
+    ss_ref = seeds.copy()
+    ref_t = o.trace_shadow(rays_s, ss_ref)
+    d_rays, d_seeds = to_dev(rays_s), to_dev(seeds.copy())
+    d_t = torch.empty((len(rays), 3), dtype=torch.float32, device="cuda")
+    pt.trace_shadow(d_rays.data_ptr(), len(rays), d_t.data_ptr(), d_seeds.data_ptr())
+    pt.synchronize()
+    assert np.array_equal(d_t.cpu().numpy(), ref_t)
+    assert np.array_equal(d_seeds.cpu().numpy(), ss_ref)
+    return ref, s_ref, ref_t, ss_ref

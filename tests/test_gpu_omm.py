@@ -5,34 +5,10 @@ import numpy as np
 import pytest
 
 from conftest import rel_rmse
+from gpu_util import trace_both
 from test_gpu_scenes import _attach, _gpu_render, _oracle
 
 pytestmark = pytest.mark.gpu
-
-
-def _trace_both(pt, o, rays, seeds, tmax=None):
-    import torch
-    from gpu_util import to_dev
-    s_ref = seeds.copy()
-    ref = o.trace_closest(rays, s_ref)
-    d_rays, d_seeds = to_dev(rays), to_dev(seeds.copy())
-    d_hits = torch.empty((len(rays), 6), dtype=torch.float32, device="cuda")
-    pt.trace_closest(d_rays.data_ptr(), len(rays), d_hits.data_ptr(), d_seeds.data_ptr())
-    pt.synchronize()
-    got = d_hits.cpu().numpy()
-    assert np.array_equal(got.view(np.uint32), ref.view(np.uint32))
-    assert np.array_equal(d_seeds.cpu().numpy(), s_ref)
-    rays_s = rays.copy()
-    rays_s[:, 7] = tmax if tmax is not None else 4.0
-    ss_ref = seeds.copy()
-    ref_t = o.trace_shadow(rays_s, ss_ref)
-    d_rays, d_seeds = to_dev(rays_s), to_dev(seeds.copy())
-    d_t = torch.empty((len(rays), 3), dtype=torch.float32, device="cuda")
-    pt.trace_shadow(d_rays.data_ptr(), len(rays), d_t.data_ptr(), d_seeds.data_ptr())
-    pt.synchronize()
-    assert np.array_equal(d_t.cpu().numpy(), ref_t)
-    assert np.array_equal(d_seeds.cpu().numpy(), ss_ref)
-    return ref, s_ref, ref_t, ss_ref
 
 
 @pytest.mark.parametrize("level", [4, 3])
@@ -54,15 +30,15 @@ def test_trace_parity_with_baked_micromaps(std_env, oracle_mod, level):
     pt, _ = _attach(scn, std_env, (16, 16))
     o = oracle_mod.Oracle()
     o.set_scene(scn)
-    ref, s_ref, ref_t, _ = _trace_both(pt, o, rays, seeds)
+    ref, s_ref, ref_t, _ = trace_both(pt, o, rays, seeds)
     assert np.array_equal(ref.view(np.uint32), h0.view(np.uint32))
     assert (s_ref != seeds).sum() < (s0 != seeds).sum()
     assert 0.02 < (ref_t[:, 0] > 0).mean() < 0.98
 
 
-def test_trace_parity_micromaps_on_deep_layers(std_env, oracle_mod):
-    """14 MASK layers with micromaps: the few UNKNOWN candidates, OPAQUE micro-triangles committing in front of or behind them,
-    continuation rounds behind a full candidate list -- closest and shadow, bit-exact, also on mirrored instances."""
+def deep_layers_with_micromaps():
+    """14 MASK layers with level-3 micromaps, two of them mirrored, and 40 000 rays through them towards the back wall.
+    Returns the scene, the bake statistics, the rays and their seeds."""
     from vk_gltf_renderer_b200 import omm, synth
     scn = synth.synth_layers(tex_size=256)
     # mirror two of the layers (negative determinant: the flattened record swaps its 2nd / 3rd vertex, TRI_FLIPPED)
@@ -72,7 +48,6 @@ def test_trace_parity_micromaps_on_deep_layers(std_env, oracle_mod):
         from vk_gltf_renderer_b200.scene import _glm
         rn["objectToWorld"], rn["worldToObject"] = _glm(m), _glm(np.linalg.inv(m))
     st = omm.bake_opacity_micromaps(scn, level=3)
-    assert st["unknown"] > 0.2 * st["micro"] and st["opaque"] > 0.03 * st["micro"] and st["transparent"] > 0.01 * st["micro"]
     rng = np.random.default_rng(11)
     n = 40000
     rays = np.zeros((n, 8), np.float32)
@@ -82,10 +57,18 @@ def test_trace_parity_micromaps_on_deep_layers(std_env, oracle_mod):
     rays[:, 4:7] = d / np.linalg.norm(d, axis=1, keepdims=True)
     rays[:, 7] = 1e32
     seeds = ((np.arange(n, dtype=np.uint64) * 40503) % (2 ** 32)).astype(np.uint32)
+    return scn, st, rays, seeds
+
+
+def test_trace_parity_micromaps_on_deep_layers(std_env, oracle_mod):
+    """14 MASK layers with micromaps: the few UNKNOWN candidates, OPAQUE micro-triangles committing in front of or behind them,
+    continuation rounds behind a full candidate list -- closest and shadow, bit-exact, also on mirrored instances."""
+    scn, st, rays, seeds = deep_layers_with_micromaps()
+    assert st["unknown"] > 0.2 * st["micro"] and st["opaque"] > 0.03 * st["micro"] and st["transparent"] > 0.01 * st["micro"]
     pt, _ = _attach(scn, std_env, (16, 16))
     o = oracle_mod.Oracle()
     o.set_scene(scn)
-    ref, s_ref, ref_t, ss_ref = _trace_both(pt, o, rays, seeds, tmax=0.7)
+    ref, s_ref, ref_t, ss_ref = trace_both(pt, o, rays, seeds, tmax=0.7)
     assert (s_ref != seeds).mean() > 0.1 and 0.01 < (ref_t[:, 0] > 0).mean() < 0.99 and (ss_ref != seeds).mean() > 0.01
 
 
@@ -134,7 +117,7 @@ def test_special_indices_and_two_state_format(std_env, oracle_mod):
         pt, _ = _attach(scn, std_env, (16, 16))
         o = oracle_mod.Oracle()
         o.set_scene(scn)
-        ref, s_ref, ref_t, ss_ref = _trace_both(pt, o, rays, seeds, tmax=3.0)
+        ref, s_ref, ref_t, ss_ref = trace_both(pt, o, rays, seeds, tmax=3.0)
         moved.append(int((s_ref != seeds).sum()))
         pt.onDetach()
     assert moved[0] == 0 and moved[1] == 0 and moved[2] > 100 and moved[3] == 0

@@ -7,6 +7,7 @@ import pytest
 
 import texref as tr
 from conftest import rel_rmse
+from gpu_util import trace_both
 from test_texture_sampling import EPS, Sweep, check_chain, compare, read_levels, reference
 from vk_gltf_renderer_b200 import tex_io
 
@@ -79,32 +80,6 @@ def test_device_sampler_matches_oracle_and_float64_reference(oracle_mod):
     pt.onDetach()
 
 
-def _trace_both(pt, o, rays, seeds):
-    import torch
-    from gpu_util import to_dev
-    s_ref = seeds.copy()
-    ref = o.trace_closest(rays, s_ref)
-    d_rays, d_seeds = to_dev(rays), to_dev(seeds.copy())
-    d_hits = torch.empty((len(rays), 6), dtype=torch.float32, device="cuda")
-    pt.trace_closest(d_rays.data_ptr(), len(rays), d_hits.data_ptr(), d_seeds.data_ptr())
-    pt.synchronize()
-    got = d_hits.cpu().numpy()
-    assert np.array_equal(got.view(np.uint32)[:, 1:4], ref.view(np.uint32)[:, 1:4])
-    assert np.array_equal(got[:, [0, 4, 5]], ref[:, [0, 4, 5]])
-    assert np.array_equal(d_seeds.cpu().numpy(), s_ref)
-    rays_s = rays.copy()
-    rays_s[:, 7] = 4.0
-    s_ref = seeds.copy()
-    ref_t = o.trace_shadow(rays_s, s_ref)
-    d_rays, d_seeds = to_dev(rays_s), to_dev(seeds.copy())
-    d_t = torch.empty((len(rays), 3), dtype=torch.float32, device="cuda")
-    pt.trace_shadow(d_rays.data_ptr(), len(rays), d_t.data_ptr(), d_seeds.data_ptr())
-    pt.synchronize()
-    assert np.array_equal(d_t.cpu().numpy(), ref_t)
-    assert np.array_equal(d_seeds.cpu().numpy(), s_ref)
-    return ref, ref_t
-
-
 def test_alpha_paths_with_every_sampler_state(oracle_mod):
     """14 stacked alpha layers, each with its own texture shape and sampler (synth.sampler_layers): the pre-gathered
     alpha records (opacityFromRecord) and, past the candidate budget, the generic getOpacity fallback decide every
@@ -117,7 +92,7 @@ def test_alpha_paths_with_every_sampler_state(oracle_mod):
     o.set_scene(scn)
     rays = random_rays(60000, [-1.6, 0.1, -2.2], [1.9, 2.1, 0.2])
     seeds = ((np.arange(len(rays), dtype=np.uint64) * 2654435761) % (2 ** 32)).astype(np.uint32)
-    ref, ref_t = _trace_both(pt, o, rays, seeds)
+    ref, _, ref_t, _ = trace_both(pt, o, rays, seeds, float_cols=(0, 4, 5))
     node = ref.view(np.int32)[:, 1]
     layer_hit = (node >= 0) & (node < 14)
     assert 0.1 < layer_hit.mean() < 0.9 and len(np.unique(node[layer_hit])) == 14

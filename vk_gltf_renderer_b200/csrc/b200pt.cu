@@ -30,6 +30,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <numeric>
 #include <string>
 #include <thread>
 #include <utility>
@@ -58,11 +59,42 @@ constexpr int kMaxIters = 4096;  // per-frame iteration counter slots
 // motion RG16F (4), depth R16F (2), specular hit distance R16F (2)
 constexpr size_t kDlssBytesPerPixel = 28;
 // Any-hit continuation rounds per bounce: a ray whose kCand candidates were all rejected goes through another k_trace / k_shadow round
-// that resumes behind the last one; after kContRoundsMax rounds whatever is still undecided finishes inside the last k_alpha.  Counter
-// arrays per lane: 5 (trace / post queues and cursors, shadow queue) + per ray kind (rounds + 1) any-hit counters, rounds continuation
-// counters and rounds continuation cursors.
+// that resumes behind the last one; after kContRoundsMax rounds whatever is still undecided finishes inside the last k_alpha.
 constexpr int kContRoundsMax = 8;
-constexpr int kCounterArrays = 5 + 2 * (3 * kContRoundsMax + 1);
+
+// The per-iteration device counters (queue sizes, dynamic-fetch cursors of the persistent walks): kArrays arrays of `stride` words, word
+// `it` of each for iteration `it` (a frame: kMaxIters bounces; the ray-level API: one).  Per ray kind (0 closest, 1 shadow): the walk's
+// cursor, the any-hit counters of round r (r = 0: the main walk's candidates), the continuation counters and cursors of round r.
+struct Counters
+{
+  uint32_t* base;
+  size_t    stride;
+  static constexpr int kPerKind = 3 * kContRoundsMax + 1;
+  static constexpr int kArrays = 5 + 2 * kPerKind;
+  uint32_t* at(int array, int it) const { return base + (size_t)array * stride + (size_t)it; }
+  uint32_t* trace(int it) const { return at(0, it); }   // closest-hit rays (k_raygen / k_shade / k_resolve append, k_trace reads)
+  uint32_t* post(int it) const { return at(1, it); }    // paths for k_resolve
+  uint32_t* shadow(int it) const { return at(4, it); }  // shadow rays
+  uint32_t* queue(int kind, int it) const { return kind ? shadow(it) : trace(it); }  // the rays a walk of this kind reads
+  uint32_t* cursor(int kind, int it) const { return at(2 + kind, it); }
+  uint32_t* anyHit(int kind, int r, int it) const { return at(5 + kind * kPerKind + r, it); }
+  uint32_t* cont(int kind, int r, int it) const { return at(5 + kind * kPerKind + kContRoundsMax + 1 + r, it); }
+  uint32_t* contCursor(int kind, int r, int it) const { return at(5 + kind * kPerKind + 2 * kContRoundsMax + 1 + r, it); }
+};
+constexpr int kCounterArrays = Counters::kArrays;
+
+// stages of the profiling events: the per-stage times and launch counts of b200pt_stats and the stage column of a B200PT_TIMELINE dump
+enum Stage : int
+{
+  kStageTrace = 0,  // closest-hit walks
+  kStageShade = 1,
+  kStageShadow = 2,  // shadow walks
+  kStageOther = 3,
+  kStageAnyHit = 4,
+  kStageResolve = 5,
+  kStageCount
+};
+constexpr const char* kStageName[kStageCount] = {"k_trace", "k_shade", "k_shadow", "other", "k_alpha", "k_resolve"};
 
 // -------------------------------------------------------------------------------------------------
 // queue helper: warp-aggregated append
@@ -1246,16 +1278,6 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_shadow(PathStat
     atomicAdd(&stats->shadowRays, (unsigned long long)count);
 }
 
-// the walk kernels have an instantiation for scenes with opacity micromaps (omm.cuh) and one without the lookup
-#define WALK_KERNEL(K, grid, ...)                  \
-  do                                               \
-  {                                                \
-    if(omm)                                        \
-      K<true><<<grid, 128, 0, st>>>(__VA_ARGS__);  \
-    else                                           \
-      K<false><<<grid, 128, 0, st>>>(__VA_ARGS__); \
-  } while(0)
-
 // ---- material-sorted shade queue (north star: "material-sorted shade queues to tame divergence") -------------------------
 // Counting sort of the bounce's path queue by the material of the hit (misses last): k_sort_count builds the histogram,
 // k_sort_scan turns it into bucket cursors, k_sort_scatter writes the queue bucket by bucket.  Histogram and offsets are
@@ -2077,7 +2099,7 @@ struct b200pt
   // scratch pool of the ray-level API (b200pt_trace_closest / b200pt_trace_shadow run the production kernels on it)
   PathState          rayP{};
   uint32_t*          rayQ[3] = {nullptr, nullptr, nullptr};  // rays, any-hit, continuation
-  uint32_t*          rayCounters = nullptr;                  // 8 words
+  uint32_t*          rayCounters = nullptr;                  // one iteration of the Counters layout
   uint32_t           rayCapacity = 0;
   DeviceArena        rayMem;
   DevStats*          dStats = nullptr;
@@ -2088,9 +2110,10 @@ struct b200pt
   struct EvRec
   {
     cudaEvent_t a, b;
-    int         cat;
+    Stage       cat;
     int         lane;  // timeline: stream the launch went to (-1 main)
     uint64_t    frame;
+    int         bounce;  // -1 outside the bounce loop
   };
   bool               profiling = false;
   // B200PT_TIMELINE=<file>: event pairs around every launch WITHOUT serialising the frames in flight; flushEvents appends
@@ -2099,8 +2122,8 @@ struct b200pt
   cudaEvent_t        tlBase = nullptr;
   std::vector<EvRec> evPool;
   size_t             evUsed = 0;
-  double             msCat[6] = {0, 0, 0, 0, 0, 0};  // 0 k_trace, 1 k_shade, 2 k_shadow, 3 other, 4 k_alpha, 5 k_resolve
-  uint64_t           launchesCat[6] = {0, 0, 0, 0, 0, 0};
+  double             msCat[kStageCount] = {};
+  uint64_t           launchesCat[kStageCount] = {};
   uint64_t           kernelLaunches = 0;
 };
 
@@ -2323,7 +2346,6 @@ void flushEvents(b200pt* h)
   if(h->evUsed == 0)
     return;
   syncAll(h);
-  static const char* const kStage[6] = {"k_trace", "k_shade", "k_shadow", "other", "k_alpha", "k_resolve"};
   for(size_t i = 0; i < h->evUsed; i++)
   {
     float ms = 0.f;
@@ -2336,12 +2358,26 @@ void flushEvents(b200pt* h)
     {
       float t0 = 0.f, t1 = 0.f;
       if(cudaEventElapsedTime(&t0, h->tlBase, h->evPool[i].a) == cudaSuccess && cudaEventElapsedTime(&t1, h->tlBase, h->evPool[i].b) == cudaSuccess)
-        fprintf(h->timeline, "%llu,%d,%s,%.4f,%.4f\n", (unsigned long long)h->evPool[i].frame, h->evPool[i].lane, kStage[h->evPool[i].cat], t0, t1);
+        fprintf(h->timeline, "%llu,%d,%s,%.4f,%.4f\n", (unsigned long long)h->evPool[i].frame, h->evPool[i].lane, kStageName[h->evPool[i].cat], t0, t1);
     }
   }
   if(h->timeline)
     fflush(h->timeline);
   h->evUsed = 0;
+}
+
+// grows the pool of profiling event pairs to n entries, up to the first failed cudaEventCreate
+cudaError_t growEventPool(b200pt* h, size_t n)
+{
+  cudaError_t e = cudaSuccess;
+  for(size_t i = h->evPool.size(); i < n && e == cudaSuccess; i++)
+  {
+    h->evPool.emplace_back();
+    e = cudaEventCreate(&h->evPool[i].a);
+    if(e == cudaSuccess)
+      e = cudaEventCreate(&h->evPool[i].b);
+  }
+  return e;
 }
 
 float srgbToLinear(float c) { return (c <= 0.04045f) ? c / 12.92f : powf((c + 0.055f) / 1.055f, 2.4f); }
@@ -2446,6 +2482,87 @@ void describeTexture(const b200pt_texture& src, const MipChain& mc, DevTex& dev)
 
 int gridFor(const b200pt* h, int perSM) { return h->numSMs * perSM; }
 
+// The launches of one frame or one ray-level call.  Every launch is counted in kernelLaunches; a timed one (a frame while profiling or
+// with B200PT_TIMELINE) is wrapped in an event pair tagged with its stage, lane, frame and bounce.
+struct Launcher
+{
+  b200pt*      h;
+  cudaStream_t stream;
+  int          lane;  // -1: the handle's stream
+  uint64_t     frame;
+  int          bounce;  // -1 outside the bounce loop
+  bool         timed;
+  uint32_t     paths;  // path slots of the wavefront
+  template <class F>
+  void operator()(Stage stage, F&& launch) const
+  {
+    if(timed)
+    {
+      if(h->evUsed == h->evPool.size())
+        flushEvents(h);
+      b200pt::EvRec& r = h->evPool[h->evUsed++];
+      r.cat = stage;
+      r.lane = lane;
+      r.frame = frame;
+      r.bounce = bounce;
+      cudaEventRecord(r.a, stream);
+      launch(stream);
+      cudaEventRecord(r.b, stream);
+    }
+    else
+      launch(stream);
+    h->kernelLaunches++;
+  }
+};
+
+// The walk of queue q (closest-hit or shadow rays) with its any-hit rounds through the any-hit and continuation queues qAlpha / qCont:
+// walk -> [k_alpha -> continuation walk] x contRounds -> k_alpha in a scene with non-opaque triangles, the bare walk otherwise.
+// baseMode is added to every launch's mode (TRACE_TMIN: closest rays of the ray-level API).
+void launchWalk(const Launcher& ctx, int shadow, const PathState& P, const uint32_t* q, uint32_t* qAlpha, uint32_t* qCont, const Counters& C, int it,
+                int baseMode)
+{
+  const b200pt*   h = ctx.h;
+  const DevScene& S = h->S;
+  // the walk kernels have an instantiation for scenes with opacity micromaps (omm.cuh) and one without the lookup
+  const bool  omm = S.bvh.ommRef != nullptr;
+  const auto  walk = shadow ? (omm ? k_shadow<true> : k_shadow<false>) : (omm ? k_trace<true> : k_trace<false>);
+  const auto  alpha = shadow ? k_alpha<true> : k_alpha<false>;
+  const Stage stage = shadow ? kStageShadow : kStageTrace;
+  const int   gA = gridFor(h, 8), gW = gridFor(h, h->walkGridPerSM), R = h->contRounds;
+  // rounds after the first see the few rays whose candidates were all rejected twice (about 1 % of a bounce); on a small wavefront
+  // a quarter-size grid keeps the fixed cost of these extra launches down (see contSmallGrid)
+  const bool  small = h->contSmallGrid < 0 ? (ctx.paths < (8u << 20)) : (h->contSmallGrid != 0);
+  ctx(stage, [&](cudaStream_t st) {
+    walk<<<gW, 128, 0, st>>>(P, S, q, C.queue(shadow, it), C.cursor(shadow, it), qAlpha, C.anyHit(shadow, 0, it), h->dStats, h->refillThreshold,
+                             h->postponeShift, baseMode);
+  });
+  if(!S.hasAlpha)
+    return;
+  for(int r = 0; r < R; r++)
+  {
+    const int gAr = (r && small) ? gridFor(h, 2) : gA, gWr = (r && small) ? gridFor(h, 2) : gW;
+    ctx(kStageAnyHit, [&](cudaStream_t st) {
+      alpha<<<gAr, 128, 2048, st>>>(P, S, qAlpha, C.anyHit(shadow, r, it), qCont, C.cont(shadow, r, it), h->dStats, baseMode | (r ? TRACE_CONT : 0));
+    });
+    ctx(stage, [&](cudaStream_t st) {
+      walk<<<gWr, 128, 0, st>>>(P, S, qCont, C.cont(shadow, r, it), C.contCursor(shadow, r, it), qAlpha, C.anyHit(shadow, r + 1, it), h->dStats,
+                                h->refillThreshold, h->postponeShift, baseMode | TRACE_CONT);
+    });
+  }
+  ctx(kStageAnyHit, [&](cudaStream_t st) { alpha<<<gA, 128, 2048, st>>>(P, S, qAlpha, C.anyHit(shadow, R, it), nullptr, nullptr, h->dStats, baseMode | TRACE_CONT); });
+}
+
+// counting sort of the queue q of a lane by KEY into qOut: k_sort_count -> k_sort_scan -> k_sort_scatter over nb buckets
+template <int KEY>
+void launchSort(const Launcher& ctx, const b200pt::Lane& L, const uint32_t* q, const uint32_t* cnt, uint32_t* qOut, uint32_t nb)
+{
+  const b200pt* h = ctx.h;
+  const int     g = gridFor(h, 4);
+  ctx(kStageOther, [&](cudaStream_t st) { k_sort_count<KEY><<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets, nb); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_sort_scan<<<1, kSortMaxBuckets, 0, st>>>(L.dBuckets, L.dBuckets + kSortMaxBuckets, nb); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_sort_scatter<KEY><<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets + kSortMaxBuckets, qOut, nb); });
+}
+
 }  // namespace
 extern "C" {
 static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count);
@@ -2546,13 +2663,7 @@ int b200pt_create(b200pt_t** out, int cuda_device)
       fprintf(h->timeline, "frame,lane,stage,start_ms,end_ms\n");
       need(cudaEventCreate(&h->tlBase));
       need(cudaEventRecord(h->tlBase, h->stream));
-      h->evPool.resize(16384);
-      for(auto& ev : h->evPool)
-      {
-        need(cudaEventCreate(&ev.a));
-        need(cudaEventCreate(&ev.b));
-        ev.cat = 3;
-      }
+      need(growEventPool(h, 16384));
     }
   }
   for(int l = 0; l < b200pt::kMaxLanes; l++)
@@ -4294,16 +4405,8 @@ int b200pt_set_profiling(b200pt_t* h, int enabled)
     return rc;
   flushEvents(h);
   h->profiling = enabled != 0;
-  if(h->profiling && h->evPool.empty())
-  {
-    h->evPool.resize(2048);
-    for(auto& e : h->evPool)
-    {
-      CK(cudaEventCreate(&e.a));
-      CK(cudaEventCreate(&e.b));
-      e.cat = 3;
-    }
-  }
+  if(h->profiling)
+    CK(growEventPool(h, 2048));
   return B200PT_OK;
 }
 
@@ -4422,141 +4525,62 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
 
   const int     laneIdx = (int)(h->frameSerial++ % (uint64_t)h->numLanes);
   b200pt::Lane& L = h->lanes[laneIdx];
-  cudaStream_t  st = L.stream;
   // the lane's pool is free once the accumulate of its previous frame ran; while profiling, frames are serialised
   // (wait for the previous frame's accumulate) so per-kernel event times are not inflated by overlap
   if(L.busy)
-    CK(cudaStreamWaitEvent(st, L.freed, 0));
+    CK(cudaStreamWaitEvent(L.stream, L.freed, 0));
   if(h->profiling && h->lastLane >= 0 && h->lastLane != laneIdx)
-    CK(cudaStreamWaitEvent(st, h->lanes[h->lastLane].freed, 0));
-  uint32_t*    cntTrace = L.dCounters;             // [kMaxIters]
-  uint32_t*    cntPost = L.dCounters + kMaxIters;  // [kMaxIters]
-  uint32_t*    workTrace = L.dCounters + 2 * kMaxIters;  // dynamic-fetch cursors of the persistent kernels
-  uint32_t*    workPost = L.dCounters + 3 * kMaxIters;
-  uint32_t*    cntShadow = L.dCounters + 4 * kMaxIters;
-  // any-hit counters of round r (r = 0: the main walk's candidates), continuation queue counters and cursors of round r, per ray kind
-  const int    R = h->contRounds;
-  auto cntA = [&](int shadow, int r) { return L.dCounters + (size_t)(5 + shadow * (3 * kContRoundsMax + 1) + r) * kMaxIters; };
-  auto cntC = [&](int shadow, int r) { return L.dCounters + (size_t)(5 + shadow * (3 * kContRoundsMax + 1) + (kContRoundsMax + 1) + r) * kMaxIters; };
-  auto wrkC = [&](int shadow, int r) { return L.dCounters + (size_t)(5 + shadow * (3 * kContRoundsMax + 1) + (2 * kContRoundsMax + 1) + r) * kMaxIters; };
-  CK(cudaMemsetAsync(L.dCounters, 0, sizeof(uint32_t) * kCounterArrays * kMaxIters, st));
-
-  enum
-  {
-    tTrace = 0,
-    tShade = 1,
-    tPost = 2,
-    tOther = 3,
-    tAnyHit = 4,
-    tResolve = 5
-  };
-  const uint64_t frameNo = h->frameSerial - 1;
-  auto timed = [&](int cat, auto&& launch) {
-    if(h->profiling || h->timeline)
-    {
-      if(h->evUsed == h->evPool.size())
-        flushEvents(h);
-      b200pt::EvRec& r = h->evPool[h->evUsed++];
-      r.cat = cat;
-      r.lane = (st == h->stream) ? -1 : laneIdx;
-      r.frame = frameNo;
-      cudaEventRecord(r.a, st);
-      launch();
-      cudaEventRecord(r.b, st);
-    }
-    else
-      launch();
-    h->kernelLaunches++;
-  };
-
+    CK(cudaStreamWaitEvent(L.stream, h->lanes[h->lastLane].freed, 0));
+  const Counters C{L.dCounters, kMaxIters};
+  CK(cudaMemsetAsync(L.dCounters, 0, sizeof(uint32_t) * kCounterArrays * kMaxIters, L.stream));
+  Launcher ctx{h, L.stream, laneIdx, h->frameSerial - 1, -1, h->profiling || h->timeline != nullptr, F.numPaths};
   const int gridWide = gridFor(h, 8);
-  timed(tOther, [&] { k_raygen<<<gridWide, 256, 0, st>>>(L.P, F, L.dQ[0], &cntTrace[0], h->dStats); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_raygen<<<gridWide, 256, 0, st>>>(L.P, F, L.dQ[0], C.trace(0), h->dStats); });
 
+  int it = 0;  // bounces run
   if(pc->maxDepth > 0)
   {
-    int       it = 0;
-    int       cur = 0;  // dQ[cur] = trace queue, dQ[2] = post queue, dQ[1-cur] = next queue
-    const int firstBatch = pc->maxDepth;
+    const int gS = gridFor(h, h->shadeGridPerSM);  // persistent shade kernel
+    const auto shade = h->featureMask == 0 ? k_shade<0u> : h->leanShade ? k_shade<FEAT_LEAN> : k_shade<FEAT_ALL>;
+    const bool        sortShade = h->sortShade && h->S.numMaterials + 1 <= kSortMaxBuckets;
+    int               cur = 0;  // dQ[cur] = trace queue, dQ[2] = post queue, dQ[1-cur] = next queue
     // (a shadowed shadow-catcher hit continues without consuming depth: such a frame can need more iterations than maxDepth)
     const bool catcherFrame = (fi->flags & B200PT_SCENE_USE_INFINITE_PLANE) && (fi->flags & B200PT_SCENE_INFINITE_PLANE_SHADOW_CATCHER);
     const bool mayOverrun = h->hasVolume || pc->numSamples > 1 || catcherFrame;
-    int        remaining = firstBatch;
+    int        remaining = pc->maxDepth;
     for(;;)
     {
       for(int k = 0; k < remaining && it < kMaxIters - 1; k++, it++)
       {
-        uint32_t* qT = L.dQ[cur];
-        uint32_t* qN = L.dQ[1 - cur];
-        // geometry walks are persistent kernels; the texture-dependent any-hit tests and the path bookkeeping run
-        // as dense one-thread-per-path kernels (k_alpha, k_resolve) sized by the device-side queue counters
-        const int gP = gridFor(h, 8);
-        const int  gW = gridFor(h, h->walkGridPerSM);  // persistent walk kernels
-        const bool smallRounds = h->contSmallGrid < 0 ? (F.numPaths < (8u << 20)) : (h->contSmallGrid != 0);
-        const int  gSmall = smallRounds ? gridFor(h, 2) : 0;  // any-hit continuation rounds after the first (0: full grids)
-        const bool omm = h->S.bvh.ommRef != nullptr;  // scenes with opacity micromaps run the walk kernels' OMM instantiation
-        const int gS = gridFor(h, h->shadeGridPerSM);  // persistent shade kernel (512-thread CTAs, one resident per SM)
-        // geometry walks are persistent kernels; the texture-dependent any-hit tests and the path bookkeeping run
-        // as dense kernels (k_alpha, k_resolve) sized by the device-side queue counters.  Any-hit: resolve kCand
-        // candidates, one continuation round for the paths that used them all up, then whatever is still
-        // undecided finishes inside the last k_alpha.
+        ctx.bounce = it;
+        uint32_t*       qT = L.dQ[cur];
+        uint32_t*       qN = L.dQ[1 - cur];
         const uint32_t* qWalk = qT;
         if(h->sortRays && it > 0)
         {
           // experiment: the trace queue bucketed by direction octant (dQ[3], the shadow queue, is free until k_shade writes it)
-          timed(tOther, [&] { k_sort_count<1><<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, qT, &cntTrace[it], L.dBuckets, 8u); });
-          timed(tOther, [&] { k_sort_scan<<<1, kSortMaxBuckets, 0, st>>>(L.dBuckets, L.dBuckets + kSortMaxBuckets, 8u); });
-          timed(tOther, [&] { k_sort_scatter<1><<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, qT, &cntTrace[it], L.dBuckets + kSortMaxBuckets, L.dQ[3], 8u); });
+          launchSort<1>(ctx, L, qT, C.trace(it), L.dQ[3], 8u);
           qWalk = L.dQ[3];
         }
-        timed(tTrace, [&] { WALK_KERNEL(k_trace, gW, L.P, h->S, qWalk, &cntTrace[it], &workTrace[it], L.dQ[4], cntA(0, 0) + it, h->dStats, h->refillThreshold, h->postponeShift, 0); });
-        if(h->S.hasAlpha)
-        {
-          for(int r = 0; r < R; r++)
-          {
-            // rounds after the first see the few rays whose candidates were all rejected TWICE (about 1 % of the bounce); on small
-            // wavefronts a quarter-size grid keeps the fixed cost of these extra launches down (see contSmallGrid)
-            const int gPr = (r && gSmall) ? gSmall : gP, gWr = (r && gSmall) ? gSmall : gW;
-            timed(tAnyHit, [&] { k_alpha<false><<<gPr, 128, 2048, st>>>(L.P, h->S, L.dQ[4], cntA(0, r) + it, L.dQ[5], cntC(0, r) + it, h->dStats, r ? TRACE_CONT : 0); });
-            timed(tTrace, [&] { WALK_KERNEL(k_trace, gWr, L.P, h->S, L.dQ[5], cntC(0, r) + it, wrkC(0, r) + it, L.dQ[4], cntA(0, r + 1) + it, h->dStats, h->refillThreshold, h->postponeShift, 1); });
-          }
-          timed(tAnyHit, [&] { k_alpha<false><<<gP, 128, 2048, st>>>(L.P, h->S, L.dQ[4], cntA(0, R) + it, nullptr, nullptr, h->dStats, TRACE_CONT); });
-        }
+        launchWalk(ctx, 0, L.P, qWalk, L.dQ[4], L.dQ[5], C, it, 0);
         const uint32_t* qShade = qT;
-        if(h->sortShade && h->S.numMaterials + 1 <= kSortMaxBuckets)
+        if(sortShade)
         {
           // dQ[4] (the any-hit queue) is free between the closest-hit any-hit kernels and the shadow walk
-          const uint32_t nb = (uint32_t)h->S.numMaterials + 1u;
-          timed(tOther, [&] { k_sort_count<0><<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, qT, &cntTrace[it], L.dBuckets, nb); });
-          timed(tOther, [&] { k_sort_scan<<<1, kSortMaxBuckets, 0, st>>>(L.dBuckets, L.dBuckets + kSortMaxBuckets, nb); });
-          timed(tOther, [&] { k_sort_scatter<0><<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, qT, &cntTrace[it], L.dBuckets + kSortMaxBuckets, L.dQ[4], nb); });
+          launchSort<0>(ctx, L, qT, C.trace(it), L.dQ[4], (uint32_t)h->S.numMaterials + 1u);
           qShade = L.dQ[4];
         }
-        timed(tShade, [&] {
-          if(h->featureMask == 0)
-            k_shade<0u><<<gS, SHADE_BLOCK, 2048, st>>>(L.P, h->S, F, qShade, &cntTrace[it], L.dQ[2], &cntPost[it], L.dQ[3], &cntShadow[it], qN, &cntTrace[it + 1], h->dStats);
-          else if(h->leanShade)
-            k_shade<FEAT_LEAN><<<gS, SHADE_BLOCK, 2048, st>>>(L.P, h->S, F, qShade, &cntTrace[it], L.dQ[2], &cntPost[it], L.dQ[3], &cntShadow[it], qN, &cntTrace[it + 1], h->dStats);
-          else
-            k_shade<FEAT_ALL><<<gS, SHADE_BLOCK, 2048, st>>>(L.P, h->S, F, qShade, &cntTrace[it], L.dQ[2], &cntPost[it], L.dQ[3], &cntShadow[it], qN, &cntTrace[it + 1], h->dStats);
+        ctx(kStageShade, [&](cudaStream_t st) {
+          shade<<<gS, SHADE_BLOCK, 2048, st>>>(L.P, h->S, F, qShade, C.trace(it), L.dQ[2], C.post(it), L.dQ[3], C.shadow(it), qN, C.trace(it + 1), h->dStats);
         });
-        timed(tPost, [&] { WALK_KERNEL(k_shadow, gW, L.P, h->S, L.dQ[3], &cntShadow[it], &workPost[it], L.dQ[4], cntA(1, 0) + it, h->dStats, h->refillThreshold, h->postponeShift, 0); });
-        if(h->S.hasAlpha)
-        {
-          for(int r = 0; r < R; r++)
-          {
-            const int gPr = (r && gSmall) ? gSmall : gP, gWr = (r && gSmall) ? gSmall : gW;
-            timed(tAnyHit, [&] { k_alpha<true><<<gPr, 128, 2048, st>>>(L.P, h->S, L.dQ[4], cntA(1, r) + it, L.dQ[5], cntC(1, r) + it, h->dStats, r ? TRACE_CONT : 0); });
-            timed(tPost, [&] { WALK_KERNEL(k_shadow, gWr, L.P, h->S, L.dQ[5], cntC(1, r) + it, wrkC(1, r) + it, L.dQ[4], cntA(1, r + 1) + it, h->dStats, h->refillThreshold, h->postponeShift, 1); });
-          }
-          timed(tAnyHit, [&] { k_alpha<true><<<gP, 128, 2048, st>>>(L.P, h->S, L.dQ[4], cntA(1, R) + it, nullptr, nullptr, h->dStats, TRACE_CONT); });
-        }
-        timed(tResolve, [&] { k_resolve<<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, F, L.dQ[2], &cntPost[it], qN, &cntTrace[it + 1], h->dStats); });
+        launchWalk(ctx, 1, L.P, L.dQ[3], L.dQ[4], L.dQ[5], C, it, 0);
+        ctx(kStageResolve, [&](cudaStream_t st) { k_resolve<<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, F, L.dQ[2], C.post(it), qN, C.trace(it + 1), h->dStats); });
         cur = 1 - cur;
       }
       if(!mayOverrun)
         break;
-      CK(cudaMemcpyAsync(L.hCount, &cntTrace[it], sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
+      CK(cudaMemcpyAsync(L.hCount, C.trace(it), sizeof(uint32_t), cudaMemcpyDeviceToHost, L.stream));
+      CK(cudaStreamSynchronize(L.stream));
       if(L.hCount[0] == 0)
         break;
       if(it >= kMaxIters - 1)
@@ -4566,54 +4590,53 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
       }
       remaining = 4;
     }
-  }
-  else
-  {
-    // maxDepth == 0: every sample is black (the while loop never runs)
+    ctx.bounce = -1;
   }
   // accumulate on the main stream, in frame order
-  CK(cudaEventRecord(L.done, st));
+  CK(cudaEventRecord(L.done, L.stream));
   CK(cudaStreamWaitEvent(h->stream, L.done, 0));
-  st = h->stream;
+  ctx.stream = h->stream;
+  ctx.lane = -1;
   if(pc->flags & B200PT_PT_FIRST_FRAME)
-    timed(tOther, [&] { k_select<<<gridFor(h, 8), 128, 0, st>>>(h->S, F, h->dSelect, h->dStats); });
-  timed(tOther, [&] { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth); });
+    ctx(kStageOther, [&](cudaStream_t st) { k_select<<<gridWide, 128, 0, st>>>(h->S, F, h->dSelect, h->dStats); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth); });
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && h->dGuide)
-    timed(tOther, [&] { k_guide<<<gridWide, 256, 0, st>>>(L.P, F, h->dGuide); });
+    ctx(kStageOther, [&](cudaStream_t st) { k_guide<<<gridWide, 256, 0, st>>>(L.P, F, h->dGuide); });
   if((pc->flags & B200PT_PT_USE_DLSS) && h->dDlss)
   {
     void*  dev[6];
     size_t bytes[6];
     dlssPlanes(h, dev, bytes);
     const DlssPlanes planes{(uint32_t*)dev[0], (uint2*)dev[1], (uint2*)dev[2], (uint32_t*)dev[3], (uint16_t*)dev[4], (uint16_t*)dev[5]};
-    timed(tOther, [&] { k_dlss_guides<<<gridWide, 256, 0, st>>>(L.P, F, planes); });
+    ctx(kStageOther, [&](cudaStream_t st) { k_dlss_guides<<<gridWide, 256, 0, st>>>(L.P, F, planes); });
   }
-  CK(cudaEventRecord(L.freed, st));
+  CK(cudaEventRecord(L.freed, h->stream));
   L.busy = true;
   h->lastLane = laneIdx;
   CK(cudaGetLastError());
   if(h->profiling && getenv("B200PT_DUMP_ITERS"))
   {
-    // tuning aid: per-iteration queue sizes and kernel times of this frame (stderr)
-    CK(cudaStreamSynchronize(st));
-    const int            n = pc->maxDepth < 64 ? pc->maxDepth : 64;
-    std::vector<uint32_t> c(2 * kMaxIters);
-    CK(cudaMemcpy(c.data(), L.dCounters, sizeof(uint32_t) * 2 * kMaxIters, cudaMemcpyDeviceToHost));
-    const size_t perIter = h->S.hasAlpha ? 11 : 5;
-    const size_t first = h->evUsed >= perIter * (size_t)pc->maxDepth + 2 ? h->evUsed - (perIter * (size_t)pc->maxDepth + 2) : 0;
-    for(int it = 0; it < n; it++)
+    // tuning aid: this frame's queue sizes and per-stage kernel times of every bounce it ran, from the events tagged with the frame and
+    // bounce, then the launches outside the bounce loop (stderr; events of the frame that a full pool flushed early are missing)
+    CK(cudaStreamSynchronize(h->stream));
+    std::vector<uint32_t> c((size_t)kCounterArrays * kMaxIters);
+    CK(cudaMemcpy(c.data(), L.dCounters, sizeof(uint32_t) * c.size(), cudaMemcpyDeviceToHost));
+    const Counters      hc{c.data(), kMaxIters};
+    std::vector<double> ms((size_t)(it + 1) * kStageCount, 0.0);  // [bounce][stage]; bounce `it`: outside the bounce loop
+    for(size_t e = 0; e < h->evUsed; e++)
     {
-      float ms[6] = {0, 0, 0, 0, 0, 0};
-      for(size_t k = 0; k < perIter; k++)
-      {
-        const size_t e = first + 1 + (size_t)it * perIter + k;
-        float        t = 0.f;
-        if(e < h->evUsed && cudaEventElapsedTime(&t, h->evPool[e].a, h->evPool[e].b) == cudaSuccess)
-          ms[h->evPool[e].cat] += t;
-      }
-      fprintf(stderr, "iter %2d  %8u rays  k_trace %.3f  k_alpha %.3f  k_shade %.3f | %8u paths  k_shadow %.3f  k_resolve %.3f ms\n", it, c[it], ms[0], ms[4], ms[1],
-              c[kMaxIters + it], ms[2], ms[5]);
+      const b200pt::EvRec& r = h->evPool[e];
+      float                t = 0.f;
+      if(r.frame == ctx.frame && cudaEventElapsedTime(&t, r.a, r.b) == cudaSuccess)
+        ms[(size_t)(r.bounce < 0 ? it : r.bounce) * kStageCount + r.cat] += t;
     }
+    for(int b = 0; b < it; b++)
+    {
+      const double* m = &ms[(size_t)b * kStageCount];
+      fprintf(stderr, "iter %2d  %8u rays  k_trace %.3f  k_alpha %.3f  k_shade %.3f | %8u shadow rays  k_shadow %.3f | %8u paths  k_resolve %.3f | other %.3f ms\n", b,
+                *hc.trace(b), m[kStageTrace], m[kStageAnyHit], m[kStageShade], *hc.shadow(b), m[kStageShadow], *hc.post(b), m[kStageResolve], m[kStageOther]);
+    }
+    fprintf(stderr, "outside the bounce loop: other %.3f ms\n", ms[(size_t)it * kStageCount + kStageOther]);
   }
   return B200PT_OK;
 }
@@ -4638,19 +4661,19 @@ int b200pt_get_stats(b200pt_t* h, b200pt_stats* out)
             (double)d.busyLaneIters / (double)d.warpIters, (double)d.nodesVisited / (double)d.warpIters, (double)d.trisTested / (double)d.warpIters);
 #endif
   flushEvents(h);
-  out->msTraceClosest = h->msCat[0];
-  out->msShade = h->msCat[1];
-  out->msTraceShadow = h->msCat[2];
-  out->msOther = h->msCat[3];
-  out->msAnyHit = h->msCat[4];
-  out->msResolve = h->msCat[5];
-  out->launchesAnyHit = h->launchesCat[4];
-  out->launchesResolve = h->launchesCat[5];
-  out->msTotal = h->msCat[0] + h->msCat[1] + h->msCat[2] + h->msCat[3] + h->msCat[4] + h->msCat[5];
+  out->msTraceClosest = h->msCat[kStageTrace];
+  out->msShade = h->msCat[kStageShade];
+  out->msTraceShadow = h->msCat[kStageShadow];
+  out->msOther = h->msCat[kStageOther];
+  out->msAnyHit = h->msCat[kStageAnyHit];
+  out->msResolve = h->msCat[kStageResolve];
+  out->msTotal = std::accumulate(std::begin(h->msCat), std::end(h->msCat), 0.0);
   out->kernelLaunches = h->kernelLaunches;
-  out->launchesTraceClosest = h->launchesCat[0];
-  out->launchesShade = h->launchesCat[1];
-  out->launchesTraceShadow = h->launchesCat[2];
+  out->launchesTraceClosest = h->launchesCat[kStageTrace];
+  out->launchesShade = h->launchesCat[kStageShade];
+  out->launchesTraceShadow = h->launchesCat[kStageShadow];
+  out->launchesAnyHit = h->launchesCat[kStageAnyHit];
+  out->launchesResolve = h->launchesCat[kStageResolve];
   return B200PT_OK;
 }
 
@@ -4662,17 +4685,14 @@ int b200pt_reset_stats(b200pt_t* h)
     return rc;
   CK(cudaMemset(h->dStats, 0, sizeof(DevStats)));
   flushEvents(h);
-  for(int k = 0; k < 6; k++)
-  {
-    h->msCat[k] = 0;
-    h->launchesCat[k] = 0;
-  }
+  std::fill(std::begin(h->msCat), std::end(h->msCat), 0.0);
+  std::fill(std::begin(h->launchesCat), std::end(h->launchesCat), 0);
   h->kernelLaunches = 0;
   return B200PT_OK;
 }
 
-// ray-level API: the rays run through the production kernels on a scratch pool (round 1 had separate restart-per-candidate
-// kernels here, so the ray-level parity tests did not cover the benchmarked code)
+// ray-level API: the rays run through the walk sequence of a frame's bounce (launchWalk: the same kernels, continuation rounds and grid
+// rule) on a scratch pool, so the ray-level parity tests check what frames run
 static int ensureRayPool(b200pt_t* h, uint32_t n)
 {
   if(n <= h->rayCapacity)
@@ -4683,7 +4703,7 @@ static int ensureRayPool(b200pt_t* h, uint32_t n)
   PathState   P;
   allocPathState(h, A, n, P);
   uint32_t* const q[3] = {A.alloc<uint32_t>(n), A.alloc<uint32_t>(n), A.alloc<uint32_t>(n)};
-  uint32_t* const counters = A.alloc<uint32_t>(8);
+  uint32_t* const counters = A.alloc<uint32_t>(kCounterArrays);
   if(!A.ok())
     return failed(h, A, "ray-level API");
   h->rayMem = std::move(A);
@@ -4704,36 +4724,15 @@ static int traceRays(b200pt_t* h, const float* dev_rays, uint32_t n, float* dev_
   const int rc = ensureRayPool(h, n);
   if(rc)
     return rc;
-  cudaStream_t st = h->stream;
-  PathState&   P = h->rayP;
-  uint32_t*    c = h->rayCounters;  // [0] rays [1] any-hit [2] continuation [3] any-hit of the continuation [4..5] work cursors
-  CK(cudaMemsetAsync(c, 0, 8 * sizeof(uint32_t), st));
-  const int  gP = gridFor(h, 8);
-  const bool omm = h->S.bvh.ommRef != nullptr;
-  k_rays_load<<<gP, 256, 0, st>>>(P, reinterpret_cast<const float4*>(dev_rays), n, dev_seeds, h->rayQ[0], &c[0], shadow);
-  if(!shadow)
-  {
-    WALK_KERNEL(k_trace, gP, P, h->S, h->rayQ[0], &c[0], &c[4], h->rayQ[1], &c[1], h->dStats, h->refillThreshold, h->postponeShift, TRACE_TMIN);
-    if(h->S.hasAlpha)
-    {
-      k_alpha<false><<<gP, 128, 2048, st>>>(P, h->S, h->rayQ[1], &c[1], h->rayQ[2], &c[2], h->dStats, TRACE_TMIN);
-      WALK_KERNEL(k_trace, gP, P, h->S, h->rayQ[2], &c[2], &c[5], h->rayQ[1], &c[3], h->dStats, h->refillThreshold, h->postponeShift, TRACE_TMIN | TRACE_CONT);
-      k_alpha<false><<<gP, 128, 2048, st>>>(P, h->S, h->rayQ[1], &c[3], nullptr, nullptr, h->dStats, TRACE_TMIN | TRACE_CONT);
-    }
-  }
-  else
-  {
-    WALK_KERNEL(k_shadow, gP, P, h->S, h->rayQ[0], &c[0], &c[4], h->rayQ[1], &c[1], h->dStats, h->refillThreshold, h->postponeShift, 0);
-    if(h->S.hasAlpha)
-    {
-      k_alpha<true><<<gP, 128, 2048, st>>>(P, h->S, h->rayQ[1], &c[1], h->rayQ[2], &c[2], h->dStats, 0);
-      WALK_KERNEL(k_shadow, gP, P, h->S, h->rayQ[2], &c[2], &c[5], h->rayQ[1], &c[3], h->dStats, h->refillThreshold, h->postponeShift, TRACE_CONT);
-      k_alpha<true><<<gP, 128, 2048, st>>>(P, h->S, h->rayQ[1], &c[3], nullptr, nullptr, h->dStats, TRACE_CONT);
-    }
-  }
-  k_rays_store<<<gP, 256, 0, st>>>(P, h->S, n, dev_out, dev_seeds, shadow);
+  const Counters C{h->rayCounters, 1};
+  CK(cudaMemsetAsync(h->rayCounters, 0, sizeof(uint32_t) * kCounterArrays, h->stream));
+  const Launcher ctx{h, h->stream, -1, 0, -1, false, n};
+  ctx(kStageOther, [&](cudaStream_t st) {
+    k_rays_load<<<gridFor(h, 8), 256, 0, st>>>(h->rayP, reinterpret_cast<const float4*>(dev_rays), n, dev_seeds, h->rayQ[0], C.queue(shadow, 0), shadow);
+  });
+  launchWalk(ctx, shadow, h->rayP, h->rayQ[0], h->rayQ[1], h->rayQ[2], C, 0, shadow ? 0 : TRACE_TMIN);
+  ctx(kStageOther, [&](cudaStream_t st) { k_rays_store<<<gridFor(h, 8), 256, 0, st>>>(h->rayP, h->S, n, dev_out, dev_seeds, shadow); });
   CK(cudaGetLastError());
-  h->kernelLaunches += h->S.hasAlpha ? 6 : 3;
   return B200PT_OK;
 }
 
