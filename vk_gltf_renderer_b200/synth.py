@@ -737,6 +737,84 @@ def triangle_soup(n, seed=1234, extent=1.0, size=0.15):
     return scn
 
 
+def icosahedron(radius=1.0):
+    """The 12 vertices (float64 [12, 3]) and 20 faces (int [20, 3], counter-clockwise seen from outside) of a regular
+    icosahedron with circumradius `radius` centred on the origin."""
+    g = (1.0 + math.sqrt(5.0)) / 2.0
+    v = np.array([[-1, g, 0], [1, g, 0], [-1, -g, 0], [1, -g, 0], [0, -1, g], [0, 1, g], [0, -1, -g], [0, 1, -g],
+                  [g, 0, -1], [g, 0, 1], [-g, 0, -1], [-g, 0, 1]], np.float64)
+    v *= radius / np.linalg.norm(v[0])
+    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2], [10, 7, 6],
+                  [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11], [6, 2, 10],
+                  [8, 6, 7], [9, 8, 1]])
+    return v, f
+
+
+def synth_furnace_polyhedron(materials, view=(0.31, 0.52, 1.0), radius=1.0):
+    """A convex icosahedron seen by an orthographic camera, for tests of the estimator's expectation.  Each of the 20 faces
+    is its own render node (node k = face k, object id k + 1) with three unshared vertices that carry the flat face normal,
+    so the shading normal is the geometric one.  `materials` is a list of add_material keyword dicts, given to the faces in
+    turn.  The orthographic camera looks along -`view`, so every pixel of a face sees it from the same direction; the body is
+    convex, so every ray leaving a face escapes to the environment and no shadow ray from a face is blocked by the body.
+    Returns (scene, face normals float64 [20, 3])."""
+    v, f = icosahedron(radius)
+    scn = Scene()
+    mats = [scn.add_material(**m) for m in materials]
+    normals = np.empty((20, 3))
+    for k, tri in enumerate(f):
+        p = v[tri]
+        n = np.cross(p[1] - p[0], p[2] - p[0])
+        n /= np.linalg.norm(n)
+        normals[k] = n
+        prim = scn.add_primitive(p, np.array([[0, 1, 2]]), normals=np.repeat(n[None], 3, 0))
+        scn.add_node(prim, mats[k % len(mats)])
+    cam = Camera()
+    cam.type = "orthographic"
+    d = np.asarray(view, np.float64) / np.linalg.norm(view)
+    cam.eye = (d * 4.0 * radius).astype(np.float32)
+    cam.center = np.zeros(3, np.float32)
+    cam.xmag = cam.ymag = 1.05 * radius
+    cam.znear, cam.zfar = 0.1 * radius, 10.0 * radius
+    scn.camera = cam
+    return scn, normals
+
+
+def synth_enclosure(rho, emission, half=1.0):
+    """A closed cube of side 2 * `half` whose six walls face inward: single-sided, emissive (`emission`, RGB) Lambertian
+    walls (base colour `rho`, metallic 0, specular 0, so the diffuse lobe is the only lobe) and a perspective camera inside.
+    Every path stays inside, so every pixel has the same expected value."""
+    scn = Scene()
+    rho = [rho] * 3 if np.isscalar(rho) else list(rho)
+    m = scn.add_material(pbrBaseColorFactor=rho + [1.0], pbrMetallicFactor=0.0, pbrRoughnessFactor=1.0, specularFactor=0.0,
+                         emissiveFactor=list(emission), doubleSided=0)
+    pos, nrm, idx = [], [], []
+    for axis in range(3):
+        for s in (-1.0, 1.0):
+            n = np.zeros(3)
+            n[axis] = -s                     # inward
+            a, b = [(axis + 1) % 3, (axis + 2) % 3]
+            quad = []
+            for u, w in ((-1, -1), (1, -1), (1, 1), (-1, 1)):
+                p = np.zeros(3)
+                p[axis], p[a], p[b] = s * half, u * half, w * half
+                quad.append(p)
+            quad = np.array(quad)
+            if np.dot(np.cross(quad[1] - quad[0], quad[2] - quad[0]), n) < 0:
+                quad = quad[::-1]
+            base = len(pos) * 4
+            pos.append(quad)
+            nrm.append(np.repeat(n[None], 4, 0))
+            idx += [[base, base + 1, base + 2], [base, base + 2, base + 3]]
+    scn.add_node(scn.add_primitive(np.concatenate(pos), np.array(idx), normals=np.concatenate(nrm)), m)
+    cam = Camera()
+    cam.eye = np.array([0.1, -0.2, 0.3], np.float32) * half
+    cam.center = np.array([0.6, 0.1, -1.0], np.float32) * half
+    cam.yfov = math.radians(70.0)
+    cam.znear, cam.zfar = 0.01 * half, 10.0 * half
+    scn.camera = cam
+    return scn
+
+
 def scene_state(scn):
     """Plain-python snapshot of a Scene (for caching generated workloads)."""
     import ctypes as C
