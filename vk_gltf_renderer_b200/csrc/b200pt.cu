@@ -233,7 +233,9 @@ __global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_consta
 // Persistent-warp scheme (Aila & Laine 2009 style): all 32 lanes of a warp reconverge at the fetch point
 // (__syncwarp), lanes that finished their ray take the next queue entries from a global cursor, then the
 // warp walks the tree until fewer than kRefillThreshold lanes are still busy and goes back to refill.
-constexpr int kRefillThresholdDefault = 22;
+constexpr int kRefillThreshold = 22;
+// 64 registers: 8 walk CTAs of 128 threads per SM (the 64 K-register file of an H100 SM full); also the walks' persistent grid
+constexpr int kWalkCtasPerSM = 8;
 
 // full-warp fetch: every lane calls it; lanes with need==true receive the next queue slot or 0xFFFFFFFF
 __device__ __forceinline__ uint32_t fetchWork(bool need, uint32_t* workCounter, uint32_t count)
@@ -262,24 +264,14 @@ __device__ __forceinline__ uint32_t fetchWork(bool need, uint32_t* workCounter, 
 // converged part of the loop, never inside the traversal loop.
 // mode: TRACE_CONT = continuation round (the paths in the queue had all kCand candidates rejected by k_alpha and resume
 // behind the last one; P.hit seeds the opaque bound and is refined), TRACE_TMIN = rayO.w carries tmin (ray-level API).
-#ifndef B200PT_TRACE_MINBLOCKS
-#define B200PT_TRACE_MINBLOCKS 8  // 64 registers: 8 blocks of 128 threads per SM (the 64 K-register file of an H100 SM full)
-#endif
-// the production walk kernels tell step() their protocol at compile time (traverse.cuh); -DB200PT_RUNTIME_MODE keeps the runtime flags (A/B)
-#ifdef B200PT_RUNTIME_MODE
-#define B200PT_STEP_MODE(m) 0
-#else
-#define B200PT_STEP_MODE(m) (m)
-#endif
 enum : int
 {
   TRACE_CONT = 1,
   TRACE_TMIN = 2,
 };
 template <bool OMM>
-__global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_trace(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
-                                                                       uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int refillThreshold,
-                                                                       int postponeShift, int mode)
+__global__ void __launch_bounds__(128, kWalkCtasPerSM) k_trace(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
+                                                               uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
 {
   __shared__ Cand s_cand[kCand * 128];  // candidate lists, one column per thread (20-byte stride: conflict-free)
   Cand* const     cand = &s_cand[threadIdx.x];
@@ -287,14 +279,7 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_trace(PathState
   const bool      cont = (mode & TRACE_CONT) != 0;
   const uint32_t  count = *cntIn;
   TravState       T;
-#ifdef B200PT_SMEM_STACK
-  __shared__ uint2 s_stack[TravState::kStackSize * 128];
-  uint2* const     stack = &s_stack[threadIdx.x];
-  constexpr int    SS = 128;
-#else
-  uint2         stack[TravState::kStackSize];
-  constexpr int SS = 1;
-#endif
+  uint2           stack[TravState::kStackSize];
   int             path = -1;
   bool            travDone = false;  // traversal finished, write-out pending
   for(;;)
@@ -367,8 +352,8 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_trace(PathState
       }
 #endif
       if(path >= 0 && !travDone)
-        travDone = T.step<SS, kCand, false, OMM, B200PT_STEP_MODE(1)>(stack, postponeShift, cand, cs, S.bvh.ommRef, S.bvh.ommData);
-      if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < refillThreshold)
+        travDone = T.step<kCand, false, OMM, 1>(stack, kPostponeShift, cand, cs, S.bvh.ommRef, S.bvh.ommData);
+      if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < kRefillThreshold)
         break;
     }
   }
@@ -603,28 +588,22 @@ __global__ void __launch_bounds__(128) k_alpha(PathState P, DevScene S, const ui
   }
 }
 
-#ifndef SHADE_BLOCK
-#define SHADE_BLOCK 256  // H100 (SynthSponza 1080p bench): 256-thread CTAs at <= 255 registers run without spills and beat 512 at <= 128
-#endif
-#ifndef SHADE_SYNC
-#define SHADE_SYNC 1  // 0: none, 1: one barrier per pass, 2: also between the four sections of a pass
-#endif
-#ifndef SHADE_MIN_BLOCKS
-#define SHADE_MIN_BLOCKS 2  // in units of 128 threads: one 256-thread block per SM
-#endif
+// H100 (SynthSponza 1080p bench): 256-thread CTAs at <= 255 registers run without spills and beat 512 at <= 128
+constexpr int kShadeBlock = 256;
+constexpr int kShadeCtasPerSM = 2;  // CTAs per SM of the persistent shade grid
 template <uint32_t FEAT>
-__global__ void __launch_bounds__(SHADE_BLOCK, SHADE_MIN_BLOCKS * 128 / SHADE_BLOCK) k_shade(PathState P, DevScene S, const __grid_constant__ FrameParams F, const uint32_t* __restrict__ q,
-                                               const uint32_t* __restrict__ cntIn, uint32_t* qPost, uint32_t* cntPost, uint32_t* qShadow, uint32_t* cntShadow,
-                                                                 uint32_t* qNext, uint32_t* cntNext, DevStats* stats)
+__global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene S, const __grid_constant__ FrameParams F, const uint32_t* __restrict__ q,
+                                                          const uint32_t* __restrict__ cntIn, uint32_t* qPost, uint32_t* cntPost, uint32_t* qShadow, uint32_t* cntShadow,
+                                                          uint32_t* qNext, uint32_t* cntNext, DevStats* stats)
 {
   stageSrgbLut(S.lutSrgb);
   const uint32_t count = *cntIn;
   const uint32_t stride = gridDim.x * blockDim.x;
   // One path per thread per pass.  The kernel is ~12 000 straight-line instructions that every warp walks once per
   // path, so it is bound by instruction fetch (ncu: no_instruction is its top stall, 20 % issue utilisation); the
-  // block-uniform loop with a barrier per pass keeps the warps of a block -- and with SHADE_BLOCK = 512 all four
-  // warps of a scheduler -- inside the same stretch of code so they share the fetched lines.
-  // pass state shared by the four sections of a pass (sections are separated by block barriers, see below)
+  // block-uniform loop with a barrier per pass keeps the eight warps of a 256-thread block inside the same stretch of
+  // code so they share the fetched lines.
+  // pass state shared by the four sections of a pass (see the pass loop below)
   uint32_t                  i = 0, flags = 0, seed = 0, scatterBounces = 0, sampleIdx = 0, depth = 0, slot = 0;
   float4                    hr, misc;
   uint4                     med;
@@ -1023,24 +1002,13 @@ __global__ void __launch_bounds__(SHADE_BLOCK, SHADE_MIN_BLOCKS * 128 / SHADE_BL
   for(uint32_t base = blockIdx.x * blockDim.x; base < count; base += stride)
   {
     bool alive = base + threadIdx.x < count;
-#if SHADE_SYNC
     __syncthreads();
-#endif
     if(alive)
       alive = shadeLoad(base + threadIdx.x);
-#if SHADE_SYNC > 1
-    __syncthreads();
-#endif
     if(alive)
       alive = shadeMaterial();
-#if SHADE_SYNC > 1
-    __syncthreads();
-#endif
     if(alive)
       alive = shadeLight();
-#if SHADE_SYNC > 1
-    __syncthreads();
-#endif
     if(alive)
       shadeBsdf();
   }
@@ -1166,9 +1134,8 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
 // the whole segment; any FORCE_OPAQUE occluder ends the query (raytracer_interface.h.slang:181-184), otherwise the kCand
 // nearest non-opaque candidates are written out for k_alpha<true>.  Same persistent-warp scheme as k_trace.
 template <bool OMM>
-__global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_shadow(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
-                                                                        uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats,
-                                                                        int refillThreshold, int postponeShift, int mode)
+__global__ void __launch_bounds__(128, kWalkCtasPerSM) k_shadow(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
+                                                                uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
 {
   __shared__ Cand s_cand[kCand * 128];
   Cand* const     cand = &s_cand[threadIdx.x];
@@ -1176,14 +1143,7 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_shadow(PathStat
   const bool      cont = (mode & TRACE_CONT) != 0;
   const uint32_t  count = *cntIn;
   TravState       T;
-#ifdef B200PT_SMEM_STACK
-  __shared__ uint2 s_stack[TravState::kStackSize * 128];
-  uint2* const     stack = &s_stack[threadIdx.x];
-  constexpr int    SS = 128;
-#else
-  uint2         stack[TravState::kStackSize];
-  constexpr int SS = 1;
-#endif
+  uint2           stack[TravState::kStackSize];
   int             path = -1;  // -1: lane needs work, -2: queue exhausted
   int             phase = 0;  // 0: occlusion query against the opaque-only tree, 1: candidates from the non-opaque tree
   bool            travDone = false;
@@ -1269,8 +1229,8 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_shadow(PathStat
       }
 #endif
       if(path >= 0 && !travDone)
-        travDone = T.step<SS, kCand, false, OMM, B200PT_STEP_MODE(2)>(stack, postponeShift, cand, cs, S.bvhA.ommRef, S.bvhA.ommData);  // (only non-opaque triangles consult it: phase 1)
-      if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < refillThreshold)
+        travDone = T.step<kCand, false, OMM, 2>(stack, kPostponeShift, cand, cs, S.bvhA.ommRef, S.bvhA.ommData);  // (only non-opaque triangles consult it: phase 1)
+      if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < kRefillThreshold)
         break;
     }
   }
@@ -1286,20 +1246,13 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_MINBLOCKS) k_shadow(PathStat
 constexpr int kSortMaxBuckets = 1024;
 constexpr int kSortItems = 4;  // paths per thread per pass
 
-// KEY 0: material of the hit (shade queue); KEY 1: direction octant of the path's next ray (trace queue, experiment B200PT_SORT_RAYS)
-template <int KEY>
+// the bucket of a path: the material of its hit, misses last
 __device__ __forceinline__ uint32_t shadeKey(const PathState& P, const DevScene& S, uint32_t path, uint32_t nb)
 {
-  if(KEY == 1)
-  {
-    const float4 d = P.rayD[path];
-    return (d.x < 0.f ? 0u : 4u) | (d.y < 0.f ? 0u : 2u) | (d.z < 0.f ? 0u : 1u);
-  }
   const uint32_t slot = __float_as_uint(P.hit[path].w);
   return slot == 0xFFFFFFFFu ? nb - 1u : min(__ldg(&S.matOfSlot[slot]), nb - 2u);
 }
 
-template <int KEY>
 __global__ void __launch_bounds__(256) k_sort_count(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn, uint32_t* bucketCount, uint32_t nb)
 {
   __shared__ uint32_t sCnt[kSortMaxBuckets];
@@ -1309,7 +1262,7 @@ __global__ void __launch_bounds__(256) k_sort_count(PathState P, DevScene S, con
   const uint32_t count = *cntIn;
   const uint32_t stride = gridDim.x * blockDim.x;
   for(uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < count; k += stride)
-    atomicAdd(&sCnt[shadeKey<KEY>(P, S, q[k], nb)], 1u);
+    atomicAdd(&sCnt[shadeKey(P, S, q[k], nb)], 1u);
   __syncthreads();
   for(uint32_t b = threadIdx.x; b < nb; b += blockDim.x)
     if(sCnt[b])
@@ -1337,7 +1290,6 @@ __global__ void __launch_bounds__(1024) k_sort_scan(uint32_t* bucketCount, uint3
   }
 }
 
-template <int KEY>
 __global__ void __launch_bounds__(256) k_sort_scatter(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn, uint32_t* bucketCursor,
                                                       uint32_t* __restrict__ qSorted, uint32_t nb)
 {
@@ -1358,7 +1310,7 @@ __global__ void __launch_bounds__(256) k_sort_scatter(PathState P, DevScene S, c
       if(k < count)
       {
         path[i] = q[k];
-        key[i] = shadeKey<KEY>(P, S, path[i], nb);
+        key[i] = shadeKey(P, S, path[i], nb);
         off[i] = atomicAdd(&sCnt[key[i]], 1u);
       }
     }
@@ -1560,7 +1512,7 @@ __global__ void __launch_bounds__(128) k_select(DevScene S, const __grid_constan
     uint2     stack[TravState::kStackSize];
     Cand      cand[1];
     T.init(S.bvh, org, dir, 0.0f, kInfinite, false, false, false, 0.f, 0u);
-    while(!T.step<1, 1, true>(stack, 2, cand, 1))
+    while(!T.step<1, true>(stack, kPostponeShift, cand, 1))
     {
     }
     if(T.overflow)
@@ -1960,7 +1912,6 @@ struct b200pt
   DeviceArena         sceneMem;  // everything b200pt_set_scene uploads, and dPrevO2W
   const void*         treeBase = nullptr;  // the trees' node + triangle arrays (one allocation) and their size: the L2 window
   size_t              treeBytes = 0;
-  int                 l2Window = 1;        // B200PT_L2_WINDOW=0: no persisting-L2 window over the trees
   // opacity micromaps as handed over by b200pt_set_opacity_micromaps (host copies; consumed by the next b200pt_set_scene)
   struct OmmHost
   {
@@ -1980,19 +1931,16 @@ struct b200pt
   bool                haveScene = false;
   uint32_t            numTextureInfos = 0;  // S.texInfos entries (host copy of the count, for argument checks)
   bool                hasVolume = false;
-  int                 refillThreshold = kRefillThresholdDefault, postponeShift = 2;  // B200PT_REFILL / B200PT_POSTPONE env overrides (tuning)
-  int                 bvhBuilder = 0;  // 0: host SAH builder (bvh.cpp), 1: device LBVH (lbvh.cuh); b200pt_set_bvh_builder / B200PT_BVH_BUILDER
+  int                 bvhBuilder = 0;  // 0: host SAH builder (bvh.cpp), 1: device LBVH (lbvh.cuh); b200pt_set_bvh_builder
   double              bvhBuildMs = 0.0;  // wall time of the last scene's tree builds
   // any-hit continuation rounds per bounce (B200PT_CONT_ROUNDS, 1..kContRoundsMax).  With one round the in-kernel fallback walks of the
   // last k_alpha (2 of 32 lanes busy) are a tail on every bounce; more rounds move that work into full-width walk launches.
-  int                 contRounds = (kCand <= 2) ? 4 : 2;
+  int                 contRounds = 2;
   // grids of the continuation rounds after the first: -1 = by wavefront size (quarter-size grids below 8 M path slots), 0 = always full,
   // 1 = always quarter-size (B200PT_CONT_SMALL_GRID).  On a small wavefront (a multi-GPU tile) an almost empty full-size walk launch
   // costs about as much as the round saves in k_alpha, hence quarter-size grids there.
   int                 contSmallGrid = -1;
-  int                 walkGridPerSM = 8, shadeGridPerSM = 2;  // CTAs per SM of the persistent walk / shade grids (B200PT_WALK_GRID, B200PT_SHADE_GRID)
-  bool                sortShade = false;
-  bool                sortRays = false;   // B200PT_SORT_RAYS=1 (experiment): trace queue bucketed by ray direction octant  // B200PT_SORT_SHADE=1: material-sorted shade queue
+  bool                sortShade = false;  // B200PT_SORT_SHADE=1: material-sorted shade queue
   bool                leanShade = false;  // scene fits the FEAT_LEAN shade variant (scene_feature_detection analogue)
   uint32_t            featureMask = 0;
   uint64_t            nodeBytes = 0, triBytes = 0;
@@ -2091,7 +2039,7 @@ struct b200pt
   int                   pendingCount = 0;
   b200pt_frame_info     pendingFi{};
   b200pt_push_constant  pendingPc{};  // the FIRST pending frame's constants
-  int                numLanes = 4;   // frames in flight (B200PT_FRAMES_IN_FLIGHT)
+  int                numLanes = 4;   // frames in flight (b200pt_set_frames_in_flight)
   uint64_t           frameSerial = 0;
   int                lastLane = -1;
   cudaEvent_t        readDone[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -2528,13 +2476,12 @@ void launchWalk(const Launcher& ctx, int shadow, const PathState& P, const uint3
   const auto  walk = shadow ? (omm ? k_shadow<true> : k_shadow<false>) : (omm ? k_trace<true> : k_trace<false>);
   const auto  alpha = shadow ? k_alpha<true> : k_alpha<false>;
   const Stage stage = shadow ? kStageShadow : kStageTrace;
-  const int   gA = gridFor(h, 8), gW = gridFor(h, h->walkGridPerSM), R = h->contRounds;
+  const int   gA = gridFor(h, 8), gW = gridFor(h, kWalkCtasPerSM), R = h->contRounds;
   // rounds after the first see the few rays whose candidates were all rejected twice (about 1 % of a bounce); on a small wavefront
   // a quarter-size grid keeps the fixed cost of these extra launches down (see contSmallGrid)
   const bool  small = h->contSmallGrid < 0 ? (ctx.paths < (8u << 20)) : (h->contSmallGrid != 0);
   ctx(stage, [&](cudaStream_t st) {
-    walk<<<gW, 128, 0, st>>>(P, S, q, C.queue(shadow, it), C.cursor(shadow, it), qAlpha, C.anyHit(shadow, 0, it), h->dStats, h->refillThreshold,
-                             h->postponeShift, baseMode);
+    walk<<<gW, 128, 0, st>>>(P, S, q, C.queue(shadow, it), C.cursor(shadow, it), qAlpha, C.anyHit(shadow, 0, it), h->dStats, baseMode);
   });
   if(!S.hasAlpha)
     return;
@@ -2546,21 +2493,20 @@ void launchWalk(const Launcher& ctx, int shadow, const PathState& P, const uint3
     });
     ctx(stage, [&](cudaStream_t st) {
       walk<<<gWr, 128, 0, st>>>(P, S, qCont, C.cont(shadow, r, it), C.contCursor(shadow, r, it), qAlpha, C.anyHit(shadow, r + 1, it), h->dStats,
-                                h->refillThreshold, h->postponeShift, baseMode | TRACE_CONT);
+                                baseMode | TRACE_CONT);
     });
   }
   ctx(kStageAnyHit, [&](cudaStream_t st) { alpha<<<gA, 128, 2048, st>>>(P, S, qAlpha, C.anyHit(shadow, R, it), nullptr, nullptr, h->dStats, baseMode | TRACE_CONT); });
 }
 
-// counting sort of the queue q of a lane by KEY into qOut: k_sort_count -> k_sort_scan -> k_sort_scatter over nb buckets
-template <int KEY>
+// counting sort of the queue q of a lane by material into qOut: k_sort_count -> k_sort_scan -> k_sort_scatter over nb buckets
 void launchSort(const Launcher& ctx, const b200pt::Lane& L, const uint32_t* q, const uint32_t* cnt, uint32_t* qOut, uint32_t nb)
 {
   const b200pt* h = ctx.h;
   const int     g = gridFor(h, 4);
-  ctx(kStageOther, [&](cudaStream_t st) { k_sort_count<KEY><<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets, nb); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_sort_count<<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets, nb); });
   ctx(kStageOther, [&](cudaStream_t st) { k_sort_scan<<<1, kSortMaxBuckets, 0, st>>>(L.dBuckets, L.dBuckets + kSortMaxBuckets, nb); });
-  ctx(kStageOther, [&](cudaStream_t st) { k_sort_scatter<KEY><<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets + kSortMaxBuckets, qOut, nb); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_sort_scatter<<<g, 256, 0, st>>>(L.P, h->S, q, cnt, L.dBuckets + kSortMaxBuckets, qOut, nb); });
 }
 
 }  // namespace
@@ -2623,26 +2569,12 @@ int b200pt_create(b200pt_t** out, int cuda_device)
     delete h;
     return B200PT_E_CUDA;
   }
-  if(const char* e = getenv("B200PT_REFILL"))
-    h->refillThreshold = atoi(e);
-  if(const char* e = getenv("B200PT_POSTPONE"))
-    h->postponeShift = atoi(e);
   if(const char* e = getenv("B200PT_SORT_SHADE"))
     h->sortShade = atoi(e) != 0;
-  if(const char* e = getenv("B200PT_L2_WINDOW"))
-    h->l2Window = atoi(e);
-  if(const char* e = getenv("B200PT_SORT_RAYS"))
-    h->sortRays = atoi(e) != 0;
-  if(const char* e = getenv("B200PT_WALK_GRID"))
-    h->walkGridPerSM = std::min(std::max(atoi(e), 1), 32);
-  if(const char* e = getenv("B200PT_SHADE_GRID"))
-    h->shadeGridPerSM = std::min(std::max(atoi(e), 1), 8);
   if(const char* e = getenv("B200PT_CONT_SMALL_GRID"))
     h->contSmallGrid = atoi(e) != 0 ? 1 : 0;
   if(const char* e = getenv("B200PT_CONT_ROUNDS"))
     h->contRounds = std::min(std::max(atoi(e), 1), kContRoundsMax);
-  if(const char* e = getenv("B200PT_BVH_BUILDER"))
-    h->bvhBuilder = (strcmp(e, "gpu") == 0 || strcmp(e, "1") == 0) ? 1 : 0;
   bool ok = true;
   auto need = [&](cudaError_t e) { ok = ok && (e == cudaSuccess); };
   cudaDeviceProp prop{};
@@ -2651,8 +2583,6 @@ int b200pt_create(b200pt_t** out, int cuda_device)
   h->dStats = h->mem.alloc<DevStats>(1);
   if(h->dStats)
     need(cudaMemset(h->dStats, 0, sizeof(DevStats)));
-  if(const char* e = getenv("B200PT_FRAMES_IN_FLIGHT"))
-    h->numLanes = std::min(std::max(atoi(e), 1), (int)b200pt::kMaxLanes);
   if(const char* e = getenv("B200PT_TIMELINE"))
   {
     // one file per process (ranks of a multi-GPU run append their pid)
@@ -3161,7 +3091,6 @@ int packTrees(b200pt* h, SceneBuild& b)
   DevScene& S = b.S;
   S.bvh.nodes = reinterpret_cast<const float4*>(dPacked);
   S.bvh.tris = reinterpret_cast<const float4*>(dPacked + offTris);
-  S.bvh.prmtPool = kPrmtPool;
   S.bvh.ommRef = nullptr;
   S.bvh.ommData = nullptr;
   S.hasAlpha = b.anyNonOpaque ? 1 : 0;
@@ -3438,7 +3367,7 @@ void commitScene(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
 // path-state traffic around them is what gets evicted).  hitRatio shrinks when the trees are larger than the carve-out.
 void setTreeWindow(b200pt* h)
 {
-  if(!h->l2Window || !h->treeBytes)
+  if(!h->treeBytes)
     return;
   int maxPersist = 0, maxWindow = 0;
   cudaDeviceGetAttribute(&maxPersist, cudaDevAttrMaxPersistingL2CacheSize, h->device);
@@ -4540,7 +4469,7 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   int it = 0;  // bounces run
   if(pc->maxDepth > 0)
   {
-    const int gS = gridFor(h, h->shadeGridPerSM);  // persistent shade kernel
+    const int gS = gridFor(h, kShadeCtasPerSM);  // persistent shade kernel
     const auto shade = h->featureMask == 0 ? k_shade<0u> : h->leanShade ? k_shade<FEAT_LEAN> : k_shade<FEAT_ALL>;
     const bool        sortShade = h->sortShade && h->S.numMaterials + 1 <= kSortMaxBuckets;
     int               cur = 0;  // dQ[cur] = trace queue, dQ[2] = post queue, dQ[1-cur] = next queue
@@ -4555,23 +4484,16 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
         ctx.bounce = it;
         uint32_t*       qT = L.dQ[cur];
         uint32_t*       qN = L.dQ[1 - cur];
-        const uint32_t* qWalk = qT;
-        if(h->sortRays && it > 0)
-        {
-          // experiment: the trace queue bucketed by direction octant (dQ[3], the shadow queue, is free until k_shade writes it)
-          launchSort<1>(ctx, L, qT, C.trace(it), L.dQ[3], 8u);
-          qWalk = L.dQ[3];
-        }
-        launchWalk(ctx, 0, L.P, qWalk, L.dQ[4], L.dQ[5], C, it, 0);
+        launchWalk(ctx, 0, L.P, qT, L.dQ[4], L.dQ[5], C, it, 0);
         const uint32_t* qShade = qT;
         if(sortShade)
         {
           // dQ[4] (the any-hit queue) is free between the closest-hit any-hit kernels and the shadow walk
-          launchSort<0>(ctx, L, qT, C.trace(it), L.dQ[4], (uint32_t)h->S.numMaterials + 1u);
+          launchSort(ctx, L, qT, C.trace(it), L.dQ[4], (uint32_t)h->S.numMaterials + 1u);
           qShade = L.dQ[4];
         }
         ctx(kStageShade, [&](cudaStream_t st) {
-          shade<<<gS, SHADE_BLOCK, 2048, st>>>(L.P, h->S, F, qShade, C.trace(it), L.dQ[2], C.post(it), L.dQ[3], C.shadow(it), qN, C.trace(it + 1), h->dStats);
+          shade<<<gS, kShadeBlock, 2048, st>>>(L.P, h->S, F, qShade, C.trace(it), L.dQ[2], C.post(it), L.dQ[3], C.shadow(it), qN, C.trace(it + 1), h->dStats);
         });
         launchWalk(ctx, 1, L.P, L.dQ[3], L.dQ[4], L.dQ[5], C, it, 0);
         ctx(kStageResolve, [&](cudaStream_t st) { k_resolve<<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, F, L.dQ[2], C.post(it), qN, C.trace(it + 1), h->dStats); });

@@ -1,8 +1,6 @@
 // bvh_stats.cpp — offline (CPU) quality check of the wide-BVH builder: traverses the compressed tree exactly like
 // the CUDA kernel (same decode, same octant order, closest-hit culling by best t) and reports nodes / triangles
-// visited per ray.  STALE=1|2|3 additionally drops stack entries the ray can no longer need (experiments for the kernel:
-// 1 = per-child entry distance kept with the entry, 2 = exact minimum over the children still in the group, 3 = one float per
-// entry, the minimum over the children left when the group was pushed).  Input: a binary dump written by scripts/dump_bvh_input.py:
+// visited per ray.  Input: a binary dump written by scripts/dump_bvh_input.py:
 //   u32 nTris, u32 nRays, nTris x 9 floats (v0,e1,e2), nRays x 8 floats (o,tmin,d,tmax)
 #include <cmath>
 #include <cstdio>
@@ -43,9 +41,8 @@ int main(int argc, char** argv)
     float id[3];
     for(int a = 0; a < 3; a++) { float d = fabsf(dir[a]) > 1e-20f ? dir[a] : copysignf(1e-20f, dir[a]); id[a] = 1.0f / d; }
     const uint32_t dsign = (dir[0] < 0 ? 0 : 1) | (dir[1] < 0 ? 0 : 2) | (dir[2] < 0 ? 0 : 4);
-    struct G { uint32_t x, y; float tn[8]; float gmin; };
-    G stack[64]; int sp = 0; G cur{0, 0x80000000u, {0, 0, 0, 0, 0, 0, 0, 0}, 0.f};
-    static const int stale = getenv("STALE") ? atoi(getenv("STALE")) : 0;
+    struct G { uint32_t x, y; };
+    G stack[64]; int sp = 0; G cur{0, 0x80000000u};
     bool hit = false;
     for(;;)
     {
@@ -53,29 +50,8 @@ int main(int argc, char** argv)
       if(cur.y & 0xff000000u)
       {
         uint32_t him = cur.y; int cb = 31 - __builtin_clz(him);
-        bool     drop = false, dropGroup = false;
-        if(stale == 1)
-          drop = cur.tn[cb - 24] > best;
-        else if(stale == 2)
-        {
-          float g = 1e38f;
-          for(int b = 24; b < 32; b++) if(him & (1u << b)) g = fminf(g, cur.tn[b - 24]);
-          dropGroup = g > best;
-        }
-        else if(stale == 3)
-          dropGroup = cur.gmin > best;
-        if(dropGroup) cur.y &= 0x00ffffffu;
-        if(drop) cur.y &= ~(1u << cb);
-        if(drop || dropGroup) { if((cur.y & 0xff000000u) == 0) { if(sp == 0) break; cur = stack[--sp]; } continue; }
         cur.y &= ~(1u << cb);
-        if(cur.y & 0xff000000u)
-        {
-          float g = 1e38f;
-          for(int b = 24; b < 32; b++) if(cur.y & (1u << b)) g = fminf(g, cur.tn[b - 24]);
-          cur.gmin = g;
-          stack[sp++] = cur;
-        }
-        cur.gmin = -1.f;  // the freshly opened node's own group is tested child by child
+        if(cur.y & 0xff000000u) stack[sp++] = cur;
         uint32_t slot = (uint32_t)(cb - 24) ^ ((him >> 8) & 7u);
         uint32_t rel = __builtin_popcount(him & ~(0xffffffffu << slot));
         const float* N = &B.nodes[(size_t)(cur.x + rel) * 20];
@@ -99,11 +75,11 @@ int main(int argc, char** argv)
             float t0 = (dir[a] < 0 ? hi : lo) * ad[a] + ao[a], t1 = (dir[a] < 0 ? lo : hi) * ad[a] + ao[a];
             tn = fmaxf(tn, t0); tf = fminf(tf, t1);
           }
-          if(tn <= tf * 1.000001f) { hm |= childBits << bitIndex; if(inner) cur.tn[bitIndex - 24] = tn; }
+          if(tn <= tf * 1.000001f) hm |= childBits << bitIndex;
         }
         cur.y = (hm & 0xff000000u) | (octInv << 8) | (eim >> 24); tg.y = hm & 0x00ffffffu;
       }
-      else { tg = cur; cur = G{0, 0, {0, 0, 0, 0, 0, 0, 0, 0}, 0.f}; }
+      else { tg = cur; cur = G{0, 0}; }
       while(tg.y)
       {
         int tb = 31 - __builtin_clz(tg.y); tg.y &= ~(1u << tb);

@@ -23,15 +23,6 @@ static inline int      __clz(uint32_t x) { return x ? __builtin_clz(x) : 32; }
 static inline int      __popc(uint32_t x) { return __builtin_popcount(x); }
 template <typename T>
 static inline T __ldg(const T* p) { return *p; }
-// PRMT: result byte i = byte (selector nibble i) of the 8-byte pool {x bytes 0..3, y bytes 4..7}
-static inline uint32_t __byte_perm(uint32_t x, uint32_t y, uint32_t s)
-{
-  const uint64_t pool = (uint64_t)x | ((uint64_t)y << 32);
-  uint32_t       r = 0;
-  for(int i = 0; i < 4; i++)
-    r |= (uint32_t)((pool >> (8 * ((s >> (4 * i)) & 7))) & 0xff) << (8 * i);
-  return r;
-}
 using std::isnan;
 using std::isinf;
 // sequential stand-ins for the atomics of the build kernels (the host harness runs the "threads" one after another)
