@@ -45,6 +45,9 @@ def lib():
         L.oracle_bsdf_sample_simple.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.oracle_bsdf_eval_simple.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.oracle_dlss_env_brdf_approx2.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_hg_sample.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_hg_pdf.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_ssa.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p]
         L.oracle_dlss_motion_vector.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.oracle_get_stats.argtypes = [C.c_void_p, C.c_void_p]
         L.oracle_reset_stats.argtypes = [C.c_void_p]
@@ -208,6 +211,27 @@ class Oracle:
         out = np.empty((len(records), 4), np.float32)
         if self.L.oracle_texture_lookup(self.h, _p(records), len(records), _p(out)):
             raise ValueError("oracle_texture_lookup: a record has a texture-info slot outside the scene or a mode other than 0 / 1")
+        return out
+
+    def hg_sample(self, records):
+        """sampleHenyeyGreenstein on float32 [n, 6] records (xi.x, xi.y, g, wi xyz) -> directions [n, 3]"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 6)
+        out = np.empty((len(records), 3), np.float32)
+        self.L.oracle_hg_sample(_p(records), len(records), _p(out))
+        return out
+
+    def hg_pdf(self, records):
+        """henyeyGreensteinPdf on float32 [n, 2] records (cos theta, g) -> [n]"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 2)
+        out = np.empty(len(records), np.float32)
+        self.L.oracle_hg_pdf(_p(records), len(records), _p(out))
+        return out
+
+    def ssa(self, rho):
+        """multiToSingleScatterAlbedo of float32 rho [n] (one channel) -> [n]"""
+        rho = np.ascontiguousarray(rho, np.float32).reshape(-1)
+        out = np.empty(len(rho), np.float32)
+        self.L.oracle_ssa(_p(rho), len(rho), _p(out))
         return out
 
     def env_brdf_approx2(self, records):

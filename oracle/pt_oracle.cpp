@@ -1557,7 +1557,9 @@ static void sampleEnvironment(const Ctx& c, float3 direction, float3& envColor, 
 
 static float computeEnvHitMisWeight(const Ctx& c, float lastSamplePdf, float envPdf)
 {
-  if(lastSamplePdf == DIRAC)
+  // an infinite pdf is a delta as well: a refraction with ior1 == ior2 sends every microfacet normal to the same direction,
+  // and the lobe's Jacobian divides by zero.  inf / (inf + x) would be NaN.
+  if(lastSamplePdf == DIRAC || std::isinf(lastSamplePdf))
     return 1.0f;
   float lw, ew;
   techniqueProbabilities(c, lw, ew);
@@ -2733,6 +2735,34 @@ int oracle_bsdf_sample_simple(const float* in, uint32_t n, float* out)
 
 // DLSS arithmetic on records: EnvBRDFApprox2 on (specular colour xyz, alpha, NoV) -> rgb; calculateMotionVector on (current xyzw,
 // previous xyzw, resolution xy) with the two view-projection matrices (glm order) -> pixel motion xy
+// Henyey-Greenstein phase function and the multiscatter-to-single-scatter albedo fit, for tests/test_phase_sampling.py
+//   oracle_hg_sample: in [n][6] (xi.x, xi.y, g, wi.xyz) -> out [n][3] sampleHenyeyGreenstein
+//   oracle_hg_pdf:    in [n][2] (cos theta, g)          -> out [n]    henyeyGreensteinPdf
+//   oracle_ssa:       in [n] rho                         -> out [n]    multiToSingleScatterAlbedo
+int oracle_hg_sample(const float* in, uint32_t n, float* out)
+{
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float* p = in + 6 * (size_t)i;
+    const float3 d = sampleHenyeyGreenstein(f2(p[0], p[1]), p[2], f3(p[3], p[4], p[5]));
+    out[3 * i + 0] = d.x;
+    out[3 * i + 1] = d.y;
+    out[3 * i + 2] = d.z;
+  }
+  return 0;
+}
+int oracle_hg_pdf(const float* in, uint32_t n, float* out)
+{
+  for(uint32_t i = 0; i < n; i++)
+    out[i] = henyeyGreensteinPdf(in[2 * i], in[2 * i + 1]);
+  return 0;
+}
+int oracle_ssa(const float* in, uint32_t n, float* out)
+{
+  for(uint32_t i = 0; i < n; i++)
+    out[i] = multiToSingleScatterAlbedo(f3(in[i])).x;
+  return 0;
+}
 int oracle_dlss_env_brdf_approx2(const float* in, uint32_t n, float* out)
 {
   for(uint32_t i = 0; i < n; i++)

@@ -707,7 +707,8 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
       const float3 edir = rotateAxis(dir, f3(0, 1, 0), -F.fi.envRotation);
       const float4 env = sampleEnvTex(S, getSphericalUv(edir));
       float        misWeight = 1.0f;
-      if(lastSamplePdf != kDirac)
+      // an infinite pdf is a delta as well (a refraction with ior1 == ior2): weight 1, not inf / inf
+      if(lastSamplePdf != kDirac && !isinf(lastSamplePdf))
       {
         float lw, ew;
         techniqueProbabilities(S, F, lw, ew);
@@ -1038,7 +1039,7 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
     if(shadowFactor.x == 1.0f && shadowFactor.y == 1.0f && shadowFactor.z == 1.0f)
     {
       float misWeight = 1.0f;
-      if(thr4.w != kDirac)
+      if(thr4.w != kDirac && !isinf(thr4.w))  // an infinite pdf is a delta as well, as in the miss branch
       {
         float lw, ew;
         techniqueProbabilities(S, F, lw, ew);

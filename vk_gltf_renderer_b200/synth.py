@@ -815,6 +815,46 @@ def synth_enclosure(rho, emission, half=1.0):
     return scn
 
 
+def synth_medium_box(material, half=(4.0, 4.0, 0.5), view=1.0):
+    """An axis-aligned box [-hx, hx] x [-hy, hy] x [-hz, hz] (`half` = (hx, hy, hz)) of one material, for tests of the
+    participating-media estimator: one render node, 24 unshared vertices carrying the outward flat normal of their face (so
+    the shading normal is the geometric one).  `material` is an add_material keyword dict; give it transmission 1,
+    metallic 0 and thicknessFactor > 0 for a medium.  An orthographic camera on +z looks down -z at the +z face over
+    [-view, view]^2, so with view < min(hx, hy) every camera ray enters the box at normal incidence through that face."""
+    hx, hy, hz = (float(h) for h in half)
+    scn = Scene()
+    m = scn.add_material(**material)
+    pos, nrm, idx = [], [], []
+    ext = (hx, hy, hz)
+    for axis in range(3):
+        for s in (-1.0, 1.0):
+            n = np.zeros(3)
+            n[axis] = s
+            a, b = (axis + 1) % 3, (axis + 2) % 3
+            quad = []
+            for u, w in ((-1, -1), (1, -1), (1, 1), (-1, 1)):
+                p = np.zeros(3)
+                p[axis], p[a], p[b] = s * ext[axis], u * ext[a], w * ext[b]
+                quad.append(p)
+            quad = np.array(quad)
+            if np.dot(np.cross(quad[1] - quad[0], quad[2] - quad[0]), n) < 0:
+                quad = quad[::-1]
+            base = len(pos) * 4
+            pos.append(quad)
+            nrm.append(np.repeat(n[None], 4, 0))
+            idx += [[base, base + 1, base + 2], [base, base + 2, base + 3]]
+    scn.add_node(scn.add_primitive(np.concatenate(pos), np.array(idx), normals=np.concatenate(nrm)), m)
+    cam = Camera()
+    cam.type = "orthographic"
+    cam.eye = np.array([0.0, 0.0, hz + 4.0], np.float32)
+    cam.center = np.array([0.0, 0.0, 0.0], np.float32)
+    cam.up = np.array([0.0, 1.0, 0.0], np.float32)
+    cam.xmag = cam.ymag = float(view)
+    cam.znear, cam.zfar = 0.1, 2.0 * hz + 8.0
+    scn.camera = cam
+    return scn
+
+
 def scene_state(scn):
     """Plain-python snapshot of a Scene (for caching generated workloads)."""
     import ctypes as C
