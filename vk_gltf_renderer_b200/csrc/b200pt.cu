@@ -123,19 +123,15 @@ __device__ __forceinline__ void statAdd(unsigned long long* p, unsigned long lon
 // -------------------------------------------------------------------------------------------------
 // camera ray + sample start (samplePixel head: gltf_pathtrace.slang:502-530; getRay: pathtrace_functions.h.slang:791-811)
 // -------------------------------------------------------------------------------------------------
-__device__ void startSample(const PathState& P, const FrameParams& F, uint32_t i, uint32_t seed, float2 jitter, uint32_t sampleIdx)
+// the pinhole or orthographic camera ray through pixel (x, y) + offset
+__device__ __forceinline__ void getRay(const FrameParams& F, uint32_t x, uint32_t y, float2 offset, float3& org, float3& dir)
 {
-  const uint32_t px = pixelOf(F, i);
-  const uint32_t x = px % (uint32_t)F.width;
-  const uint32_t y = pixelRow(F, px);
-  const Mat4&    projI = *reinterpret_cast<const Mat4*>(F.fi.projInv);
-  const Mat4&    viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
-  const bool     ortho = (F.fi.flags & B200PT_SCENE_IS_ORTHOGRAPHIC) != 0;
-  const float2   clip = f2(((float)x + jitter.x) / F.fi.imageSize[0] * 2.0f - 1.0f, ((float)y + jitter.y) / F.fi.imageSize[1] * 2.0f - 1.0f);
-  float4         vc = mul_vM(f4(clip.x, clip.y, -1.0f, 1.0f), projI);
+  const Mat4&  projI = *reinterpret_cast<const Mat4*>(F.fi.projInv);
+  const Mat4&  viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
+  const float2 clip = f2(((float)x + offset.x) / F.fi.imageSize[0] * 2.0f - 1.0f, ((float)y + offset.y) / F.fi.imageSize[1] * 2.0f - 1.0f);
+  float4       vc = mul_vM(f4(clip.x, clip.y, -1.0f, 1.0f), projI);
   vc = vc / vc.w;
-  float3 org, dir;
-  if(ortho)
+  if(F.fi.flags & B200PT_SCENE_IS_ORTHOGRAPHIC)
   {
     org = xyz(mul_vM(vc, viewI));
     dir = normalize(xyz(mul_vM(f4(0, 0, -1, 0), viewI)));
@@ -144,6 +140,17 @@ __device__ void startSample(const PathState& P, const FrameParams& F, uint32_t i
   {
     org = f3(viewI.m[12], viewI.m[13], viewI.m[14]);
     dir = normalize(xyz(mul_vM(vc, viewI)) - org);
+  }
+}
+
+__device__ void startSample(const PathState& P, const FrameParams& F, uint32_t i, uint32_t seed, float2 jitter, uint32_t sampleIdx)
+{
+  const uint32_t px = pixelOf(F, i);
+  float3         org, dir;
+  getRay(F, px % (uint32_t)F.width, pixelRow(F, px), jitter, org, dir);
+  if(!(F.fi.flags & B200PT_SCENE_IS_ORTHOGRAPHIC))
+  {
+    const Mat4& viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
     // thin-lens DOF: the two rand() are consumed even when aperture == 0 (:519-520)
     const float3 focalPoint = dir * F.pc.focalDistance;
     const float  cam_r1 = rnd(seed) * kTwoPi;
@@ -236,6 +243,8 @@ __global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_consta
 constexpr int kRefillThreshold = 22;
 // 64 registers: 8 walk CTAs of 128 threads per SM (the 64 K-register file of an H100 SM full); also the walks' persistent grid
 constexpr int kWalkCtasPerSM = 8;
+// threads per walk CTA, also the column stride of the walks' shared candidate lists
+constexpr int kWalkBlock = 128;
 
 // full-warp fetch: every lane calls it; lanes with need==true receive the next queue slot or 0xFFFFFFFF
 __device__ __forceinline__ uint32_t fetchWork(bool need, uint32_t* workCounter, uint32_t count)
@@ -255,29 +264,17 @@ __device__ __forceinline__ uint32_t fetchWork(bool need, uint32_t* workCounter, 
   return k < count ? k : 0xFFFFFFFFu;
 }
 
-// IRaytracer::Trace, geometry part, for every path in the queue: ONE walk of the scene tree gives the closest
-// FORCE_OPAQUE hit and the kCand nearest any-hit candidates in front of it (traverse.cuh).  The stochastic alpha
-// tests need textures and touch only the few lanes whose walk just ended -- inside this kernel they ran with ~2 of
-// 32 lanes active and took a large share of its instructions and stall samples -- so they live in
-// the dense kernel k_alpha; this kernel only writes the candidates out.
-// Per lane: path (-1 needs work, -2 exhausted) and a resumable traversal; finished lanes are handled in the
-// converged part of the loop, never inside the traversal loop.
-// mode: TRACE_CONT = continuation round (the paths in the queue had all kCand candidates rejected by k_alpha and resume
-// behind the last one; P.hit seeds the opaque bound and is refined), TRACE_TMIN = rayO.w carries tmin (ray-level API).
-enum : int
+// The persistent-warp loop of the walk kernels, over the `count` paths of queue q.  Per lane: path (-1 needs work, -2
+// exhausted) and a resumable traversal; finished lanes are handled in the converged part of the loop, never inside the
+// traversal loop.  start(T, path) begins the walk of a fetched path; finish(T, cand, path) writes a finished walk out and
+// returns whether the lane is free (false: it started T again on the same path).  OMM, MODE and omm are those of
+// TravState::step (MODE 1: closest-hit walk, 2: shadow walk); a continuation round (cont) does not count its rays again.
+template <bool OMM, int MODE, class Start, class Finish>
+__device__ __forceinline__ void walkQueue(const uint32_t* __restrict__ q, uint32_t count, uint32_t* workCounter, const BvhView& omm, DevStats* stats, bool cont,
+                                          Start start, Finish finish)
 {
-  TRACE_CONT = 1,
-  TRACE_TMIN = 2,
-};
-template <bool OMM>
-__global__ void __launch_bounds__(128, kWalkCtasPerSM) k_trace(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
-                                                               uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
-{
-  __shared__ Cand s_cand[kCand * 128];  // candidate lists, one column per thread (20-byte stride: conflict-free)
+  __shared__ Cand s_cand[kCand * kWalkBlock];  // candidate lists, one column per thread (20-byte stride: conflict-free)
   Cand* const     cand = &s_cand[threadIdx.x];
-  constexpr int   cs = 128;
-  const bool      cont = (mode & TRACE_CONT) != 0;
-  const uint32_t  count = *cntIn;
   TravState       T;
   uint2           stack[TravState::kStackSize];
   int             path = -1;
@@ -289,24 +286,11 @@ __global__ void __launch_bounds__(128, kWalkCtasPerSM) k_trace(PathState P, DevS
     {
       travDone = false;
       T.flushCounters(&stats->nodesVisited, &stats->trisTested);
-      const TraceHit ho = T.result();
-      P.hit[path] = f4(ho.t, ho.u, ho.v, __uint_as_float(ho.slot));
-      const int n = T.candidatesInFront(cand, cs);
-      if(n > 0)
-      {
-#pragma unroll
-        for(int i = 0; i < kCand; i++)
-          if(i < n)
-          {
-            const Cand c = cand[i * cs];
-            P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
-          }
-        P.candInfo[path] = make_uint2((uint32_t)n, cand[(n - 1) * cs].gid);
-        queuePush(qAlpha, cntAlpha, (uint32_t)path);
-      }
-      if(T.overflow)
+      const bool overflow = T.overflow;  // (finish may start T again)
+      if(finish(T, cand, path))
+        path = -1;
+      if(overflow)
         atomicOr(&stats->errorFlags, 1ull);
-      path = -1;
     }
     __syncwarp();
     // ---- refill ----
@@ -320,18 +304,7 @@ __global__ void __launch_bounds__(128, kWalkCtasPerSM) k_trace(PathState P, DevS
         else
         {
           path = (int)q[k];
-          const float4 o = P.rayO[path];
-          const float4 d = P.rayD[path];
-          const float  tmin = (mode & TRACE_TMIN) ? o.w : 0.0f;
-          if(!cont)
-            T.init(S.bvh, xyz(o), xyz(d), tmin, d.w, true, false, false, 0.f, 0u);
-          else
-          {
-            T.init(S.bvh, xyz(o), xyz(d), tmin, d.w, true, false, true, P.cand[kCand - 1][path].x, P.candInfo[path].y);
-            const float4 hp = P.hit[path];
-            if(__float_as_uint(hp.w) != 0xFFFFFFFFu)
-              T.seedOpaque(hp.x, hp.y, hp.z, __float_as_uint(hp.w));
-          }
+          start(T, path);
         }
       }
     }
@@ -352,13 +325,65 @@ __global__ void __launch_bounds__(128, kWalkCtasPerSM) k_trace(PathState P, DevS
       }
 #endif
       if(path >= 0 && !travDone)
-        travDone = T.step<kCand, false, OMM, 1>(stack, kPostponeShift, cand, cs, S.bvh.ommRef, S.bvh.ommData);
+        travDone = T.step<kCand, false, OMM, MODE>(stack, kPostponeShift, cand, kWalkBlock, omm.ommRef, omm.ommData);
       if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < kRefillThreshold)
         break;
     }
   }
   if(blockIdx.x == 0 && threadIdx.x == 0 && !cont)
-    atomicAdd(&stats->closestRays, (unsigned long long)count);
+    atomicAdd(MODE == 1 ? &stats->closestRays : &stats->shadowRays, (unsigned long long)count);
+}
+
+// IRaytracer::Trace, geometry part, for every path in the queue: ONE walk of the scene tree gives the closest
+// FORCE_OPAQUE hit and the kCand nearest any-hit candidates in front of it (traverse.cuh).  The stochastic alpha
+// tests need textures and touch only the few lanes whose walk just ended -- inside this kernel they ran with ~2 of
+// 32 lanes active and took a large share of its instructions and stall samples -- so they live in
+// the dense kernel k_alpha; this kernel only writes the candidates out.
+// mode: TRACE_CONT = continuation round (the paths in the queue had all kCand candidates rejected by k_alpha and resume
+// behind the last one; P.hit seeds the opaque bound and is refined), TRACE_TMIN = rayO.w carries tmin (ray-level API).
+enum : int
+{
+  TRACE_CONT = 1,
+  TRACE_TMIN = 2,
+};
+template <bool OMM>
+__global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_trace(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
+                                                                      uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
+{
+  const bool cont = (mode & TRACE_CONT) != 0;
+  auto       start = [&](TravState& T, int path) {
+    const float4 o = P.rayO[path];
+    const float4 d = P.rayD[path];
+    const float  tmin = (mode & TRACE_TMIN) ? o.w : 0.0f;
+    if(!cont)
+      T.init(S.bvh, xyz(o), xyz(d), tmin, d.w, true, false, false, 0.f, 0u);
+    else
+    {
+      T.init(S.bvh, xyz(o), xyz(d), tmin, d.w, true, false, true, P.cand[kCand - 1][path].x, P.candInfo[path].y);
+      const float4 hp = P.hit[path];
+      if(__float_as_uint(hp.w) != 0xFFFFFFFFu)
+        T.seedOpaque(hp.x, hp.y, hp.z, __float_as_uint(hp.w));
+    }
+  };
+  auto finish = [&](TravState& T, const Cand* cand, int path) {
+    const TraceHit ho = T.result();
+    P.hit[path] = f4(ho.t, ho.u, ho.v, __uint_as_float(ho.slot));
+    const int n = T.candidatesInFront(cand, kWalkBlock);
+    if(n > 0)
+    {
+#pragma unroll
+      for(int i = 0; i < kCand; i++)
+        if(i < n)
+        {
+          const Cand c = cand[i * kWalkBlock];
+          P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
+        }
+      P.candInfo[path] = make_uint2((uint32_t)n, cand[(n - 1) * kWalkBlock].gid);
+      queuePush(qAlpha, cntAlpha, (uint32_t)path);
+    }
+    return true;
+  };
+  walkQueue<OMM, 1>(q, *cntIn, workCounter, S.bvh, stats, cont, start, finish);
 }
 
 // Any-hit part of IRaytracer::Trace (SHADOW = false) and IRaytracer::TraceShadow (SHADOW = true): the candidates
@@ -380,6 +405,15 @@ __global__ void __launch_bounds__(128) k_alpha(PathState P, DevScene S, const ui
   // the split opaque / non-opaque arrays for shadow rays
   const uint2* __restrict__ triMeta = SHADOW ? S.triMetaS : S.triMeta;
   constexpr int             KF = 16;  // candidates per walk of the in-kernel fallback (its list lives in local memory)
+  // the opacity of a candidate of the fallback walks, and its (u, v) with a mirrored instance's swap undone
+  auto fallbackOpacity = [&](const Cand& c, float& u, float& v) {
+    const uint2               meta = triMeta[c.slot];
+    const bool                flip = ((meta.x >> 28) & TRI_FLIPPED) != 0;
+    u = flip ? c.v : c.u;
+    v = flip ? c.u : c.v;
+    const b200pt_render_node& node = S.nodes[meta.x & 0x0fffffffu];
+    return getOpacity(S, node, S.prims[node.renderPrimID], meta.y, f3(1.0f - u - v, u, v));
+  };
   stageSrgbLut(S.lutSrgb);
   const uint32_t count = *cntIn;
   constexpr int  G = kCand, PPW = 32 / kCand;  // lanes per path, paths per warp
@@ -455,11 +489,8 @@ __global__ void __launch_bounds__(128) k_alpha(PathState P, DevScene S, const ui
           const int m = walkCollect<KF>(S.bvh, xyz(o), xyz(d), tmin, d.w, true, false, true, true, loT, loId, opq, cand, &overflowed);
           for(int i = 0; i < m && !accepted; i++)
           {
-            const uint2               meta = triMeta[cand[i].slot];
-            const bool                flip = ((meta.x >> 28) & TRI_FLIPPED) != 0;
-            const float               u = flip ? cand[i].v : cand[i].u, v = flip ? cand[i].u : cand[i].v;
-            const b200pt_render_node& node = S.nodes[meta.x & 0x0fffffffu];
-            const float               opacity = getOpacity(S, node, S.prims[node.renderPrimID], meta.y, f3(1.0f - u - v, u, v));
+            float       u, v;
+            const float opacity = fallbackOpacity(cand[i], u, v);
             if(rnd(seed) <= opacity)
             {
               if(sub == 0)
@@ -561,11 +592,8 @@ __global__ void __launch_bounds__(128) k_alpha(PathState P, DevScene S, const ui
           }
           for(int i = 0; i < m && !done; i++)
           {
-            const uint2               meta = triMeta[cand[i].slot];
-            const bool                flip = ((meta.x >> 28) & TRI_FLIPPED) != 0;
-            const float               u = flip ? cand[i].v : cand[i].u, v = flip ? cand[i].u : cand[i].v;
-            const b200pt_render_node& node = S.nodes[meta.x & 0x0fffffffu];
-            const float               opacity = getOpacity(S, node, S.prims[node.renderPrimID], meta.y, f3(1.0f - u - v, u, v));
+            float       u, v;
+            const float opacity = fallbackOpacity(cand[i], u, v);
             if(rnd(seed) < opacity)
               accept(cand[i].slot, cand[i].t, u, v);
           }
@@ -586,6 +614,22 @@ __global__ void __launch_bounds__(128) k_alpha(PathState P, DevScene S, const ui
     if(valid && sub == 0 && seed != seedIn)
       reinterpret_cast<uint32_t*>(&P.misc[path])[3] = seed;
   }
+}
+
+// the infinite plane's material, gltf_pathtrace.slang:169-173: defaultPbrMaterial(infinitePlaneBaseColor, metallic, roughness, N, N)
+// (nvshaders, external: restated -- GGX alpha = roughness^2 like evaluateMaterial, tangent frame from the normal; same in the oracle)
+__device__ __forceinline__ PbrMaterial planeMaterial(const FrameParams& F)
+{
+  const float3 n = f3(0, 1, 0);
+  PbrMaterial  m = defaultPbrMaterial();
+  m.baseColor = f3(F.fi.infinitePlaneBaseColor[0], F.fi.infinitePlaneBaseColor[1], F.fi.infinitePlaneBaseColor[2]);
+  m.metallic = F.fi.infinitePlaneMetallic;
+  const float r = F.fi.infinitePlaneRoughness;
+  m.roughness = f2(r * r, r * r);
+  m.N = m.Ng = m.Nc = n;
+  m.T = xyz(makeFastTangent(n));
+  m.B = cross(m.N, m.T);
+  return m;
 }
 
 // H100 (SynthSponza 1080p bench): 256-thread CTAs at <= 255 registers run without spills and beat 512 at <= 128
@@ -704,17 +748,8 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
         sp->y = (sp->y & 0xffffu) | ((uint32_t)dlssHalfBits(65504.0f) << 16);
         flags &= ~PF_SPEC_CAPTURE;
       }
-      const float3 edir = rotateAxis(dir, f3(0, 1, 0), -F.fi.envRotation);
-      const float4 env = sampleEnvTex(S, getSphericalUv(edir));
-      float        misWeight = 1.0f;
-      // an infinite pdf is a delta as well (a refraction with ior1 == ior2): weight 1, not inf / inf
-      if(lastSamplePdf != kDirac && !isinf(lastSamplePdf))
-      {
-        float lw, ew;
-        techniqueProbabilities(S, F, lw, ew);
-        misWeight = lastSamplePdf / (lastSamplePdf + ew * env.w);
-      }
-      radiance += throughput * misWeight * (xyz(env) * F.fi.envIntensity);
+      const float4 env = sampleEnvironment(S, F, dir);
+      radiance += throughput * computeEnvHitMisWeight(S, F, lastSamplePdf, env.w) * xyz(env);
       finalizeSample(P, F, i, radiance, (flags & PF_SOLID) != 0, seed, sampleIdx, qNext, cntNext, stats);
       return false;
     }
@@ -742,18 +777,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     int unlit = 0;
     if(onPlane)
     {
-      // gltf_pathtrace.slang:169-173: defaultPbrMaterial(infinitePlaneBaseColor, metallic, roughness, N, N) (nvshaders, external:
-      // restated -- GGX alpha = roughness^2 like evaluateMaterial, tangent frame from the normal; same in the oracle)
-      pbrMat = defaultPbrMaterial();
-      pbrMat.baseColor = f3(F.fi.infinitePlaneBaseColor[0], F.fi.infinitePlaneBaseColor[1], F.fi.infinitePlaneBaseColor[2]);
-      pbrMat.metallic = F.fi.infinitePlaneMetallic;
-      const float r = F.fi.infinitePlaneRoughness;
-      pbrMat.roughness = f2(r * r, r * r);
-      pbrMat.N = hit.nrm;
-      pbrMat.Ng = hit.nrm;
-      pbrMat.Nc = hit.nrm;
-      pbrMat.T = xyz(makeFastTangent(hit.nrm));
-      pbrMat.B = cross(pbrMat.N, pbrMat.T);
+      pbrMat = planeMaterial(F);
       if(F.fi.flags & B200PT_SCENE_INFINITE_PLANE_SHADOW_CATCHER)
       {
         // gltf_pathtrace.slang:175-186: the catcher returns before the first-hit captures, the roughness clamp and emission; its light
@@ -830,6 +854,20 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
 
     return true;
   };
+  // the end of sections 3 and 4: the path's next ray and state
+  auto storePath = [&]() {
+    P.rayO[i] = f4(org, coneWidth);
+    P.rayD[i] = f4(normalize(dir), kInfinite);
+    P.thr[i] = f4(throughput, lastSamplePdf);
+    P.rad[i] = f4(radiance, __uint_as_float(scatterBounces));
+    P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
+  };
+  // the path goes on to k_resolve, and its pending shadow ray to the shadow walk
+  auto handOff = [&]() {
+    queuePush(qPost, cntPost, i);
+    if(flags & PF_SHADOW_VALID)
+      queuePush(qShadow, cntShadow, i);
+  };
   // ---- section 3: in-volume segment, light / environment sample ----
   auto shadeLight = [&]() -> bool {
     flags &= ~(PF_POST_VOLUME | PF_SHADOW_VALID | PF_SHADOW_INSIDE);
@@ -885,14 +923,8 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
           throughput *= expv(ext * -hitT);
         if(scattered)
         {
-          P.rayO[i] = f4(org, coneWidth);
-          P.rayD[i] = f4(normalize(dir), kInfinite);
-          P.thr[i] = f4(throughput, lastSamplePdf);
-          P.rad[i] = f4(radiance, __uint_as_float(scatterBounces));
-          P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
-          queuePush(qPost, cntPost, i);
-          if(flags & PF_SHADOW_VALID)
-            queuePush(qShadow, cntShadow, i);
+          storePath();
+          handOff();
           return false;
         }
       }
@@ -916,9 +948,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
       }
       P.rayO[i] = f4(hit.pos, coneWidth);  // the incoming direction stays in rayD: the second half looks the environment up along it
       P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
-      queuePush(qPost, cntPost, i);
-      if(flags & PF_SHADOW_VALID)
-        queuePush(qShadow, cntShadow, i);
+      handOff();
       return false;
     }
     nextEventValid = (dot(directLight.direction, hit.nrm) > 0.0f || pbrMat.diffuseTransmissionFactor > 0.0f) && directLight.pdf != 0.0f;
@@ -990,15 +1020,9 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     }
 
     flags = (flags & ~PF_DEPTH_MASK) | (depth & PF_DEPTH_MASK);
-    P.rayO[i] = f4(org, coneWidth);
-    P.rayD[i] = f4(normalize(dir), kInfinite);
-    P.thr[i] = f4(throughput, lastSamplePdf);
-    P.rad[i] = f4(radiance, __uint_as_float(scatterBounces));
-    P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
+    storePath();
     P.medium[i] = med;
-    queuePush(qPost, cntPost, i);
-    if(flags & PF_SHADOW_VALID)
-      queuePush(qShadow, cntShadow, i);
+    handOff();
   };
   for(uint32_t base = blockIdx.x * blockDim.x; base < count; base += stride)
   {
@@ -1026,6 +1050,7 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
   float3       radiance = xyz(rad4);
   const float4 thr4 = P.thr[i];
   float3       throughput = xyz(thr4);
+  auto         endSample = [&]() { finalizeSample(P, F, i, radiance, (flags & PF_SOLID) != 0, seed, P.medium[i].w >> 16, qNext, cntNext, stats); };
   if(flags & PF_CATCHER)
   {
     // handleShadowCatcher, second half (pathtrace_functions.h.slang:525-553): lit plane points show the environment behind them and
@@ -1033,41 +1058,26 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
     const float3 shadowFactor = haveShadow ? xyz(P.shC[i]) * Tfac : f3(1.0f);
     const float4 ro = P.rayO[i];
     const float3 hitPos = xyz(ro), dir = xyz(P.rayD[i]);
-    const float4 env = sampleEnvTex(S, getSphericalUv(rotateAxis(dir, f3(0, 1, 0), -F.fi.envRotation)));
-    const float3 envColor = xyz(env) * F.fi.envIntensity;
+    const float4 env = sampleEnvironment(S, F, dir);
+    const float3 envColor = xyz(env);
     flags &= ~(PF_CATCHER | PF_POST_VOLUME | PF_SHADOW_VALID | PF_SHADOW_INSIDE);
     if(shadowFactor.x == 1.0f && shadowFactor.y == 1.0f && shadowFactor.z == 1.0f)
     {
-      float misWeight = 1.0f;
-      if(thr4.w != kDirac && !isinf(thr4.w))  // an infinite pdf is a delta as well, as in the miss branch
-      {
-        float lw, ew;
-        techniqueProbabilities(S, F, lw, ew);
-        misWeight = thr4.w / (thr4.w + ew * env.w);
-      }
-      radiance += throughput * misWeight * envColor;
-      finalizeSample(P, F, i, radiance, (flags & PF_SOLID) != 0, seed, P.medium[i].w >> 16, qNext, cntNext, stats);
+      radiance += throughput * computeEnvHitMisWeight(S, F, thr4.w, env.w) * envColor;
+      endSample();
       return;
     }
     radiance += envColor * shadowFactor;
     radiance -= envColor * (f3(1.0f) - shadowFactor) * F.fi.shadowCatcherDarkenAmount;
-    PbrMaterial  pm = defaultPbrMaterial();  // the plane's material, as k_shade built it (gltf_pathtrace.slang:169-173)
-    const float3 n = f3(0, 1, 0);
-    pm.baseColor = f3(F.fi.infinitePlaneBaseColor[0], F.fi.infinitePlaneBaseColor[1], F.fi.infinitePlaneBaseColor[2]);
-    pm.metallic = F.fi.infinitePlaneMetallic;
-    const float r = F.fi.infinitePlaneRoughness;
-    pm.roughness = f2(r * r, r * r);
-    pm.N = pm.Ng = pm.Nc = n;
-    pm.T = xyz(makeFastTangent(n));
-    pm.B = cross(pm.N, pm.T);
-    const float      a = rnd(seed), b = rnd(seed), c = rnd(seed);
-    const BsdfSample sd = bsdfSampleSimple(pm, -dir, f3(a, b, c));
+    const PbrMaterial pm = planeMaterial(F);
+    const float       a = rnd(seed), b = rnd(seed), c = rnd(seed);
+    const BsdfSample  sd = bsdfSampleSimple(pm, -dir, f3(a, b, c));
     if(sd.event_type == BSDF_EVENT_ABSORB)
     {
-      finalizeSample(P, F, i, radiance, (flags & PF_SOLID) != 0, seed, P.medium[i].w >> 16, qNext, cntNext, stats);
+      endSample();
       return;
     }
-    const float3 offsetDir = dot(sd.k2, n) > 0 ? n : -n;
+    const float3 offsetDir = dot(sd.k2, pm.N) > 0 ? pm.N : -pm.N;
     throughput *= sd.bsdf_over_pdf;
     P.rayO[i] = f4(safeOffsetRay(hitPos, offsetDir), ro.w);
     P.rayD[i] = f4(normalize(sd.k2), kInfinite);
@@ -1079,53 +1089,35 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
   }
   if(haveShadow)
     radiance += xyz(P.shC[i]) * Tfac;
-  uint32_t     depth = flags & PF_DEPTH_MASK;
-  bool         alive = true, thrDirty = false;
-  if(flags & PF_POST_VOLUME)
+  uint32_t depth = flags & PF_DEPTH_MASK;
+  // Russian roulette: inside a volume only after VOLUME_FREE_BUDGET scatters (pathtrace_functions.h.slang:925-931), on a surface
+  // from depth 3 (gltf_pathtrace.slang:476-485)
+  const bool volume = (flags & PF_POST_VOLUME) != 0;
+  const bool roulette = volume ? __float_as_uint(rad4.w) >= 64u : depth >= 3u;
+  bool       alive = true;
+  if(roulette)
   {
-    // in-volume Russian roulette only after VOLUME_FREE_BUDGET scatters (pathtrace_functions.h.slang:925-931)
-    if(__float_as_uint(rad4.w) >= 64u)
-    {
-      const float rrPcont = fminf(maxc(throughput) + 0.001f, 0.95f);
-      if(rnd(seed) >= rrPcont)
-        alive = false;
-      else
-      {
-        throughput /= rrPcont;
-        thrDirty = true;
-      }
-    }
+    const float rrPcont = fminf(maxc(throughput) + 0.001f, 0.95f);
+    if(rnd(seed) >= rrPcont)
+      alive = false;
+    else
+      throughput /= rrPcont;
   }
-  else
+  if(alive && !volume)
   {
-    // surface Russian roulette from depth 3 (gltf_pathtrace.slang:476-485)
-    if(depth >= 3u)
-    {
-      const float rrPcont = fminf(maxc(throughput) + 0.001f, 0.95f);
-      if(rnd(seed) >= rrPcont)
-        alive = false;
-      else
-      {
-        throughput /= rrPcont;
-        thrDirty = true;
-      }
-    }
-    if(alive)
-    {
-      depth++;
-      if((int)depth >= F.pc.maxDepth)
-        alive = false;
-    }
+    depth++;
+    if((int)depth >= F.pc.maxDepth)
+      alive = false;
   }
   if(!alive)
   {
-    finalizeSample(P, F, i, radiance, (flags & PF_SOLID) != 0, seed, P.medium[i].w >> 16, qNext, cntNext, stats);
+    endSample();
     return;
   }
   flags = (flags & ~(PF_DEPTH_MASK | PF_POST_VOLUME | PF_SHADOW_VALID | PF_SHADOW_INSIDE)) | (depth & PF_DEPTH_MASK);
   if(haveShadow)
     P.rad[i] = f4(radiance, rad4.w);
-  if(thrDirty)
+  if(roulette)
     P.thr[i] = f4(throughput, thr4.w);
   P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
   queuePush(qNext, cntNext, i);
@@ -1134,109 +1126,61 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
 // IRaytracer::TraceShadow, geometry part, for every path with a pending NEE shadow ray: ONE walk of the scene tree along
 // the whole segment; any FORCE_OPAQUE occluder ends the query (raytracer_interface.h.slang:181-184), otherwise the kCand
 // nearest non-opaque candidates are written out for k_alpha<true>.  Same persistent-warp scheme as k_trace.
+// candInfo.x of a shadow ray that an opaque occluder ended (raytracer_interface.h.slang:181-184)
+constexpr uint32_t kShadowOccluded = 0x80000000u;
 template <bool OMM>
-__global__ void __launch_bounds__(128, kWalkCtasPerSM) k_shadow(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
-                                                                uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
+__global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_shadow(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
+                                                                       uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
 {
-  __shared__ Cand s_cand[kCand * 128];
-  Cand* const     cand = &s_cand[threadIdx.x];
-  constexpr int   cs = 128;
-  const bool      cont = (mode & TRACE_CONT) != 0;
-  const uint32_t  count = *cntIn;
-  TravState       T;
-  uint2           stack[TravState::kStackSize];
-  int             path = -1;  // -1: lane needs work, -2: queue exhausted
-  int             phase = 0;  // 0: occlusion query against the opaque-only tree, 1: candidates from the non-opaque tree
-  bool            travDone = false;
-  for(;;)
-  {
-    __syncwarp();
-    if(path >= 0 && travDone)
+  const bool cont = (mode & TRACE_CONT) != 0;
+  int        phase = 0;  // 0: occlusion query against the opaque-only tree, 1: candidates from the non-opaque tree
+  auto       start = [&](TravState& T, int path) {
+    const float4 so = P.shO[path];
+    const float4 sd = P.shD[path];
+    if(!cont)
     {
-      travDone = false;
-      T.flushCounters(&stats->nodesVisited, &stats->trisTested);
-      if(T.overflow)
-        atomicOr(&stats->errorFlags, 1ull);
-      if(phase == 0 && T.best.slot == 0xFFFFFFFFu && S.hasAlpha)
-      {
-        // no opaque occluder: the non-opaque candidates of the segment, nearest first
-        // With opacity micromaps an OPAQUE micro-triangle anywhere on the segment ends the query like a FORCE_OPAQUE occluder
-        // (a committed hit, raytracer_interface.h.slang:181-184), so the walk must not stop looking behind the 4th candidate.
-        phase = 1;
-        T.init(S.bvhA, T.org, T.dir, 0.0f, T.tmax, false, true, false, 0.f, 0u, !OMM);
-      }
-      else
-      {
-        uint2 info = make_uint2(0u, 0u);
-        if(T.best.slot != 0xFFFFFFFFu)
-          info.x = 0x80000000u;  // an opaque occluder ended the query (raytracer_interface.h.slang:181-184)
-        else
-        {
-          const int n = T.collectN;
+      phase = 0;
+      T.init(S.bvhO, xyz(so), xyz(sd), 0.0f, so.w, false, true, false, 0.f, 0u, false);
+    }
+    else
+    {
+      phase = 1;
+      T.init(S.bvhA, xyz(so), xyz(sd), 0.0f, so.w, false, true, true, P.cand[kCand - 1][path].x, P.candInfo[path].y, true);
+    }
+  };
+  auto finish = [&](TravState& T, const Cand* cand, int path) {
+    if(phase == 0 && T.best.slot == 0xFFFFFFFFu && S.hasAlpha)
+    {
+      // no opaque occluder: the non-opaque candidates of the segment, nearest first
+      // With opacity micromaps an OPAQUE micro-triangle anywhere on the segment ends the query like a FORCE_OPAQUE occluder
+      // (a committed hit, raytracer_interface.h.slang:181-184), so the walk must not stop looking behind the 4th candidate.
+      phase = 1;
+      T.init(S.bvhA, T.org, T.dir, 0.0f, T.tmax, false, true, false, 0.f, 0u, !OMM);
+      return false;
+    }
+    uint2 info = make_uint2(0u, 0u);
+    if(T.best.slot != 0xFFFFFFFFu)
+      info.x = kShadowOccluded;
+    else
+    {
+      const int n = T.collectN;
 #pragma unroll
-          for(int i = 0; i < kCand; i++)
-            if(i < n)
-            {
-              const Cand c = cand[i * cs];
-              P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
-            }
-          info = make_uint2((uint32_t)n, n > 0 ? cand[(n - 1) * cs].gid : 0u);
-        }
-        P.candInfo[path] = info;
-        // (a continuation path always goes back to k_alpha: its running transmission is parked and must be folded)
-        if((info.x != 0u && info.x != 0x80000000u) || cont)
-          queuePush(qAlpha, cntAlpha, (uint32_t)path);
-        path = -1;
-      }
-    }
-    __syncwarp();
-    {
-      const bool     need = (path == -1);
-      const uint32_t k = fetchWork(need, workCounter, count);
-      if(need)
-      {
-        if(k == 0xFFFFFFFFu)
-          path = -2;
-        else
+      for(int i = 0; i < kCand; i++)
+        if(i < n)
         {
-          path = (int)q[k];
-          const float4 so = P.shO[path];
-          const float4 sd = P.shD[path];
-          if(!cont)
-          {
-            phase = 0;
-            T.init(S.bvhO, xyz(so), xyz(sd), 0.0f, so.w, false, true, false, 0.f, 0u, false);
-          }
-          else
-          {
-            phase = 1;
-            T.init(S.bvhA, xyz(so), xyz(sd), 0.0f, so.w, false, true, true, P.cand[kCand - 1][path].x, P.candInfo[path].y, true);
-          }
+          const Cand c = cand[i * kWalkBlock];
+          P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
         }
-      }
+      info = make_uint2((uint32_t)n, n > 0 ? cand[(n - 1) * kWalkBlock].gid : 0u);
     }
-    if(__all_sync(0xffffffffu, path == -2))
-      break;
-    for(;;)
-    {
-#ifdef B200PT_COUNT_TRAVERSAL
-      {
-        const unsigned busy = __ballot_sync(0xffffffffu, path >= 0 && !travDone);
-        if((threadIdx.x & 31) == 0)
-        {
-          atomicAdd(&stats->warpIters, 1ull);
-          atomicAdd(&stats->busyLaneIters, (unsigned long long)__popc(busy));
-        }
-      }
-#endif
-      if(path >= 0 && !travDone)
-        travDone = T.step<kCand, false, OMM, 2>(stack, kPostponeShift, cand, cs, S.bvhA.ommRef, S.bvhA.ommData);  // (only non-opaque triangles consult it: phase 1)
-      if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < kRefillThreshold)
-        break;
-    }
-  }
-  if(blockIdx.x == 0 && threadIdx.x == 0 && !cont)
-    atomicAdd(&stats->shadowRays, (unsigned long long)count);
+    P.candInfo[path] = info;
+    // (a continuation path always goes back to k_alpha: its running transmission is parked and must be folded)
+    if((info.x != 0u && info.x != kShadowOccluded) || cont)
+      queuePush(qAlpha, cntAlpha, (uint32_t)path);
+    return true;
+  };
+  // (only the non-opaque triangles of phase 1 consult the micromaps)
+  walkQueue<OMM, 2>(q, *cntIn, workCounter, S.bvhA, stats, cont, start, finish);
 }
 
 // ---- material-sorted shade queue (north star: "material-sorted shade queues to tame divergence") -------------------------
@@ -1344,7 +1288,7 @@ __global__ void __launch_bounds__(256) k_resolve(PathState P, DevScene S, const 
     const uint32_t seed = __float_as_uint(misc.w);
     const bool     haveShadow = (flags & PF_SHADOW_VALID) != 0;
     float3         vis = f3(1.0f);
-    if(haveShadow && (P.candInfo[path].x & 0x80000000u))
+    if(haveShadow && (P.candInfo[path].x & kShadowOccluded))
       vis = f3(0.0f);
 #ifdef B200PT_DEBUG
     if(haveShadow && (float)(pixelOf(F, path) % (uint32_t)F.width) == F.pc.mouseCoord[0] && (float)pixelRow(F, pixelOf(F, path)) == F.pc.mouseCoord[1])
@@ -1488,27 +1432,10 @@ __global__ void __launch_bounds__(256) k_snapshot_prev_transforms(const b200pt_r
 __global__ void __launch_bounds__(128) k_select(DevScene S, const __grid_constant__ FrameParams F, uint32_t* __restrict__ objectId, DevStats* stats)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
-  const Mat4&    projI = *reinterpret_cast<const Mat4*>(F.fi.projInv);
-  const Mat4&    viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
-  const bool     ortho = (F.fi.flags & B200PT_SCENE_IS_ORTHOGRAPHIC) != 0;
   for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels; i += stride)
   {
-    const uint32_t x = i % (uint32_t)F.width;
-    const uint32_t y = pixelRow(F, i);
-    const float2   clip = f2(((float)x + 0.5f) / F.fi.imageSize[0] * 2.0f - 1.0f, ((float)y + 0.5f) / F.fi.imageSize[1] * 2.0f - 1.0f);
-    float4         vc = mul_vM(f4(clip.x, clip.y, -1.0f, 1.0f), projI);
-    vc = vc / vc.w;
     float3 org, dir;
-    if(ortho)
-    {
-      org = xyz(mul_vM(vc, viewI));
-      dir = normalize(xyz(mul_vM(f4(0, 0, -1, 0), viewI)));
-    }
-    else
-    {
-      org = f3(viewI.m[12], viewI.m[13], viewI.m[14]);
-      dir = normalize(xyz(mul_vM(vc, viewI)) - org);
-    }
+    getRay(F, i % (uint32_t)F.width, pixelRow(F, i), f2(0.5f, 0.5f), org, dir);
     TravState T;
     uint2     stack[TravState::kStackSize];
     Cand      cand[1];
@@ -1701,7 +1628,7 @@ __global__ void __launch_bounds__(256) k_rays_store(PathState P, DevScene S, uin
     if(shadow)
     {
       const float4 c = P.shC[i];
-      const bool   occluded = (P.candInfo[i].x & 0x80000000u) != 0;
+      const bool   occluded = (P.candInfo[i].x & kShadowOccluded) != 0;
       out[i * 3] = occluded ? 0.0f : c.x;
       out[i * 3 + 1] = occluded ? 0.0f : c.y;
       out[i * 3 + 2] = occluded ? 0.0f : c.z;

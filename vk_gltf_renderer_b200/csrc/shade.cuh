@@ -745,6 +745,25 @@ PT_D void techniqueProbabilities(const DevScene& S, const FrameParams& F, float&
   }
 }
 
+// the environment along world direction `direction`: radiance (xyz, times envIntensity) and pdf (w)
+PT_D float4 sampleEnvironment(const DevScene& S, const FrameParams& F, float3 direction)
+{
+  const float4 env = sampleEnvTex(S, getSphericalUv(rotateAxis(direction, f3(0, 1, 0), -F.fi.envRotation)));
+  return f4(xyz(env) * F.fi.envIntensity, env.w);
+}
+
+// MIS weight of a path that hit the environment after a BSDF or phase sample of pdf lastSamplePdf
+PT_D float computeEnvHitMisWeight(const DevScene& S, const FrameParams& F, float lastSamplePdf, float envPdf)
+{
+  // an infinite pdf is a delta as well: a refraction with ior1 == ior2 sends every microfacet normal to the same direction,
+  // and the lobe's Jacobian divides by zero.  inf / (inf + x) would be NaN.
+  if(lastSamplePdf == kDirac || isinf(lastSamplePdf))
+    return 1.0f;
+  float lw, ew;
+  techniqueProbabilities(S, F, lw, ew);
+  return lastSamplePdf / (lastSamplePdf + ew * envPdf);
+}
+
 template <uint32_t FEAT>
 PT_D DirectLight sampleLights(const DevScene& S, const FrameParams& F, float3 pos, uint32_t& seed)
 {
@@ -783,10 +802,7 @@ PT_D DirectLight sampleLights(const DevScene& S, const FrameParams& F, float3 po
       dl.direction = rotateAxis(dl.direction, f3(0, 1, 0), F.fi.envRotation);
     }
     else
-    {
-      const float3 dir = rotateAxis(dl.direction, f3(0, 1, 0), -F.fi.envRotation);
-      envPdf = sampleEnvTex(S, getSphericalUv(dir)).w;
-    }
+      envPdf = sampleEnvironment(S, F, dl.direction).w;
   }
   float misWeight = 1.0f;
   if(dl.pdf != kDirac)
