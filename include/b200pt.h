@@ -381,6 +381,26 @@ typedef struct b200pt_node_hierarchy
 int b200pt_set_node_hierarchy(b200pt_t* h, const b200pt_node_hierarchy* hierarchy);
 int b200pt_update_node_matrices(b200pt_t* h, const float* local_matrices);
 
+/* Scene edits without a rebuild of the scene (GltfRenderer::updateSceneChanges, src/renderer.cpp:2269-2362).  After any sequence
+ * of edits the handle renders exactly what a fresh handle renders when b200pt_set_scene gets the edited description (same BVH
+ * builder, same animation / hierarchy / micromap calls).  Each call first launches a pending frame batch and waits for the frames
+ * in flight; every check runs before the first device write, so a refused call (or B200PT_E_NOMEM) leaves the scene as it was.
+ * Accumulation is not reset (restart it with frameCount, as after a transform update).  The trees are rewritten in place when the
+ * visible set stays and no visible triangle changes between opaque and any-hit; otherwise they are rebuilt with the handle's
+ * builder from the primitives' current vertices and the nodes' current transforms (an animated pose stays).  Synchronous.
+ *
+ * b200pt_update_materials: both tables, as MaterialCache::buildFromMaterials produces them (num_materials must be the scene's;
+ *   the texture-info count may change, the texture images may not).  Checked like b200pt_set_scene's materials.
+ * b200pt_update_node_materials: every render node's materialID (-1 = material 0), the KHR_materials_variants switch
+ *   (Scene::setCurrentVariant); also rewrites the node hierarchy's mappings, which b200pt_update_node_matrices applies.
+ * b200pt_update_lights: the light array; the count may change.
+ * b200pt_set_node_visibility: one flag per render node, as b200pt_scene_desc::renderNodeVisible. */
+int b200pt_update_materials(b200pt_t* h, const b200pt_shade_material* materials, uint32_t num_materials, const b200pt_texture_info* texture_infos,
+                            uint32_t num_texture_infos);
+int b200pt_update_node_materials(b200pt_t* h, const int32_t* material_ids, uint32_t num_nodes);
+int b200pt_update_lights(b200pt_t* h, const b200pt_light* lights, uint32_t num_lights);
+int b200pt_set_node_visibility(b200pt_t* h, const uint8_t* visible, uint32_t num_nodes);
+
 /* Animation feed, deforming part: morph-target blending and skeletal skinning of render primitives' vertex arrays ON THE DEVICE
  * (shaders/morph.comp.slang:29-70, shaders/skinning.comp.slang:27-70, push constants shaders/animation_io.h.slang:29-59), as
  * SceneAnimationVk::createAnimationResources / cmdUpdateAnimation drive them (src/gltf_scene_animation_vk.cpp:120-260, 396-592).

@@ -21,6 +21,7 @@ EXPORTS = [
     "b200pt_read_selection", "b200pt_get_selection_device", "b200pt_set_frame_batch", "b200pt_flush", "b200pt_update_transforms", "b200pt_set_bvh_builder", "b200pt_bvh_build_ms",
     "b200pt_set_opacity_micromaps", "b200pt_set_animation", "b200pt_animate", "b200pt_set_node_hierarchy", "b200pt_update_node_matrices", "b200pt_tonemap", "b200pt_tonemap_image", "b200pt_get_tonemapped_device", "b200pt_set_guide_outputs", "b200pt_read_guide", "b200pt_get_guide_device",
     "b200pt_set_dlss_guides", "b200pt_read_dlss_guides", "b200pt_get_dlss_guides_device",
+    "b200pt_update_materials", "b200pt_update_node_materials", "b200pt_update_lights", "b200pt_set_node_visibility",
 ]
 
 
@@ -86,6 +87,10 @@ def lib(count_traversal=False):
     L.b200pt_animate.argtypes = [vp, vp, vp, vp]
     L.b200pt_set_node_hierarchy.argtypes = [vp, C.POINTER(abi.NodeHierarchy)]
     L.b200pt_update_node_matrices.argtypes = [vp, vp]
+    L.b200pt_update_materials.argtypes = [vp, C.POINTER(abi.ShadeMaterial), u32, C.POINTER(abi.TextureInfo), u32]
+    L.b200pt_update_node_materials.argtypes = [vp, C.POINTER(C.c_int32), u32]
+    L.b200pt_update_lights.argtypes = [vp, C.POINTER(abi.Light), u32]
+    L.b200pt_set_node_visibility.argtypes = [vp, C.POINTER(C.c_uint8), u32]
     L.b200pt_tonemap.argtypes = [vp, C.POINTER(abi.Tonemapper), vp, C.c_size_t, C.POINTER(C.c_float)]
     L.b200pt_tonemap_image.argtypes = [vp, C.POINTER(abi.Tonemapper), vp, i32, i32, vp, C.POINTER(C.c_float)]
     L.b200pt_get_tonemapped_device.argtypes = [vp, C.POINTER(vp), C.POINTER(C.c_size_t)]

@@ -17,6 +17,7 @@
 //   morph.comp / skinning.comp                     shaders/*.comp.slang                  -> k_morph, k_skin, k_regather_shade (animate.cuh)
 //   world_matrix_propagate / update_render_instances                                     -> k_propagate_level, k_update_render_nodes
 //   BLAS / TLAS build and update                   src/gltf_scene_rtx.cpp:173-503        -> k_lbvh_* (lbvh.cuh), k_refit_* (refit.cuh)
+//   updateSceneChanges: material edits             src/renderer.cpp:2269-2362            -> k_retag_tris, k_gather_alpha (or a tree rebuild)
 //   GltfRenderer::tonemap                          src/renderer.cpp:992-1054             -> k_tm_histogram, k_tm_exposure, k_tonemap (tonemap.cuh)
 // One path slot per pixel; samples of a pixel within a frame run back to back in the same slot
 // (path regeneration) because the reference continues ONE rng stream across a pixel's samples.
@@ -1590,6 +1591,43 @@ __global__ void __launch_bounds__(256) k_regather_shade(ShadeRec* recs, DevPrim 
     regatherShadeRec(recs + t, P, t);
 }
 
+// ---- in-place scene edits (b200pt_update_materials / b200pt_update_node_materials): the tables changed, no triangle changed
+// TRI_OPAQUE, so the trees' shapes stay and only what the materials decide is rewritten -------------------------------------
+// the flag nibble of every triangle record (and its triMeta copy) from its node's material, TRI_FLIPPED kept; with matOfSlot,
+// also the slot's material index
+__global__ void __launch_bounds__(256) k_retag_tris(float* tris, uint2* triMeta, uint32_t* matOfSlot, uint32_t n, const b200pt_render_node* nodes,
+                                                    const b200pt_shade_material* mats)
+{
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
+  {
+    float*         T = tris + (size_t)i * 12;
+    const uint32_t w0 = __float_as_uint(T[3]), rnode = w0 & 0x0fffffffu;
+    const uint32_t mat = materialOf(nodes[rnode]);
+    const uint32_t w = rnode | ((triFlags(mats[mat]) | ((w0 >> 28) & TRI_FLIPPED)) << 28);
+    T[3] = __uint_as_float(w);
+    triMeta[i].x = w;
+    if(matOfSlot)
+      matOfSlot[i] = mat;
+  }
+}
+
+// the alpha-test records of the non-opaque triangles (slots base .. base + n - 1 of the shadow rays' triangle array)
+__global__ void __launch_bounds__(256) k_gather_alpha(AlphaRec* recs, const uint2* __restrict__ metaS, uint32_t base, uint32_t n, DevScene S)
+{
+  const uint32_t stride = gridDim.x * blockDim.x;
+  for(uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n; k += stride)
+  {
+    const uint2                meta = metaS[base + k];
+    const b200pt_render_node&  node = S.nodes[meta.x & 0x0fffffffu];
+    const DevPrim              P = S.prims[node.renderPrimID];
+    const DevTex*              tex = S.textures;
+    auto                       level0 = [tex](int t) { return tex[t].texels + tex[t].levelOfs[0]; };
+    recs[k] = alphaRecOf(S.mats[materialOf(node)], S.texInfos, tex, (uint32_t)S.numTextures, level0, P.uv0, P.uv1, P.col, P.idx[meta.y * 3],
+                         P.idx[meta.y * 3 + 1], P.idx[meta.y * 3 + 2]);
+  }
+}
+
 // ---- ray-level API (parity tests / traversal micro-benchmark): the rays run through the PRODUCTION kernels
 // (k_trace / k_shadow -> k_alpha -> continuation round -> k_alpha) on a scratch path pool -------------------------
 __global__ void __launch_bounds__(256) k_rays_load(PathState P, const float4* __restrict__ rays, uint32_t n, const uint32_t* __restrict__ seeds, uint32_t* q, uint32_t* cnt,
@@ -1837,7 +1875,18 @@ struct b200pt
   DeviceArena  mem;           // dStats, dLutSrgb, dTmHist and the lanes' counters and buckets
 
   // scene
-  DeviceArena         sceneMem;  // everything b200pt_set_scene uploads, and dPrevO2W
+  DeviceArena         sceneMem;  // what b200pt_set_scene uploads that no scene edit replaces, and dPrevO2W
+  DeviceArena         treeMem;   // the trees and every per-slot table over them: what a rebuild after a scene edit replaces
+  DeviceArena         tableMem;  // S.mats and S.texInfos (b200pt_update_materials replaces them)
+  DeviceArena         lightMem;  // S.lights (b200pt_update_lights)
+  // host copies of what the scene edits compare against or rebuild from
+  std::vector<b200pt_shade_material> materials;
+  std::vector<b200pt_texture_info>   texInfos;
+  std::vector<uint8_t>               visible;    // per render node
+  std::vector<DevTex>                devTex;     // S.textures ...
+  std::vector<const uchar4*>         texLevel0;  // ... and their level-0 texels
+  AlphaRec*                          dAlphaRecsW = nullptr;  // == S.alphaRecs, writable
+  uint32_t*                          dMatOfSlotW = nullptr;  // == S.matOfSlot, writable
   const void*         treeBase = nullptr;  // the trees' node + triangle arrays (one allocation) and their size: the L2 window
   size_t              treeBytes = 0;
   // opacity micromaps as handed over by b200pt_set_opacity_micromaps (host copies; consumed by the next b200pt_set_scene)
@@ -2169,8 +2218,18 @@ void freeScene(b200pt* h)
   h->renderedSinceUpdate = false;
   h->anim = b200pt::Animation{};
   h->graph = b200pt::Hierarchy{};
+  h->treeMem.release();
+  h->tableMem.release();
+  h->lightMem.release();
   h->sceneMem.release();
   h->primHost.clear();
+  h->materials.clear();
+  h->texInfos.clear();
+  h->visible.clear();
+  h->devTex.clear();
+  h->texLevel0.clear();
+  h->dAlphaRecsW = nullptr;
+  h->dMatOfSlotW = nullptr;
   h->dShadeRecsW = nullptr;
   h->dNodesW = nullptr;
   h->dPrimsW = nullptr;
@@ -2611,15 +2670,17 @@ namespace {
 // what b200pt_set_scene builds before it hands the scene to the handle
 struct SceneBuild
 {
-  DeviceArena                   mem;
+  DeviceArena                   mem, treeMem, tableMem, lightMem;  // the handle's arenas of the same names (sceneMem = mem)
   DevScene                      S{};
   b200pt_render_node*           nodesW = nullptr;  // == S.nodes, writable
   ShadeRec*                     shadeRecsW = nullptr;  // == S.shadeRecs, writable
+  AlphaRec*                     alphaRecsW = nullptr;  // == S.alphaRecs, writable
+  uint32_t*                     matOfSlotW = nullptr;  // == S.matOfSlot, writable
   std::vector<b200pt::PrimHost> primHost;
   std::vector<DevTex>           devTex;     // host copies of the texture records ...
   std::vector<const uchar4*>    texLevel0;  // ... and their level-0 texels (device), for the alpha-triangle records
   std::vector<FlatTri>          flat;
-  bool                          hasVolume = false, anyNonOpaque = false;
+  bool                          anyNonOpaque = false;
   WideBvh                       bvh, bvhO, bvhA;
   double                        bvhBuildMs = 0.0;
   const void*                   treeBase = nullptr;
@@ -2629,15 +2690,63 @@ struct SceneBuild
   uint32_t                      ommTriangles = 0;
 };
 
-// the instance flags of a material's triangles (getInstanceFlag, src/gltf_scene_rtx.cpp:271-295)
-uint32_t triFlags(const b200pt_shade_material& m)
+// the checks of a material table against a texture-info table of numTextureInfos entries (b200pt_set_scene and
+// b200pt_update_materials; `who` names the call in the message)
+int validateMaterials(b200pt* h, const char* who, const b200pt_shade_material* mats, uint32_t numMaterials, uint32_t numTextureInfos)
 {
-  uint32_t flags = 0;
-  if(m.transmissionFactor == 0.0f && m.alphaMode == 0 && m.diffuseTransmissionFactor == 0.0f)
-    flags |= TRI_OPAQUE;
-  if(m.doubleSided == 1 || m.thicknessFactor > 0.0f || m.transmissionFactor > 0.0f)
-    flags |= TRI_NOCULL;
-  return flags;
+  for(uint32_t i = 0; i < numMaterials; i++)
+  {
+    const b200pt_shade_material& m = mats[i];
+    // the 22 texture slots index GltfTextureInfo[] (0 = none, shaders/gltf_scene_io.h.slang:196-219)
+    const uint16_t* slots = &m.pbrBaseColorTexture;
+    for(int k = 0; k < 22; k++)
+      if(slots[k] != 0 && slots[k] >= numTextureInfos)
+      {
+        h->err = std::string(who) + ": material texture slot beyond numTextureInfos";
+        return B200PT_E_INVALID;
+      }
+    if(m.retroreflectionFactor > 0.0f)
+    {
+      h->err = std::string(who) + ": KHR_materials_retroreflection is not built (its lobe lives in nvshaders, external to the reference tree)";
+      return B200PT_E_UNSUPPORTED;
+    }
+  }
+  return B200PT_OK;
+}
+
+// a visible render node whose material puts its triangles into the any-hit path exists (render nodes already checked)
+bool anyNonOpaqueOf(const b200pt_scene_desc& s)
+{
+  for(uint32_t n = 0; n < s.numRenderNodes; n++)
+  {
+    const b200pt_render_node& node = s.renderNodes[n];
+    if((!s.renderNodeVisible || s.renderNodeVisible[n]) && s.renderPrimitives[node.renderPrimID].triangleCount
+       && !(triFlags(s.materials[materialOf(node)]) & TRI_OPAQUE))
+      return true;
+  }
+  return false;
+}
+
+// the micromaps are linked only into scenes with non-opaque triangles (linkMicromaps): then every linked primitive must be covered
+int validateMicromaps(b200pt* h, const char* who, const b200pt_scene_desc& s)
+{
+  if(!anyNonOpaqueOf(s))
+    return B200PT_OK;
+  for(const auto& po : h->primOmms)
+  {
+    if(po.prim >= s.numRenderPrimitives)
+    {
+      h->err = std::string(who) + ": opacity micromap linked to a render primitive out of range";
+      return B200PT_E_INVALID;
+    }
+    const uint32_t nTri = s.renderPrimitives[po.prim].triangleCount;
+    if(po.hasIdx ? po.idx.size() < nTri : (uint64_t)po.base + nTri > h->omms[po.micromap].tris.size())
+    {
+      h->err = std::string(who) + ": opacity micromap does not cover its primitive's triangles";
+      return B200PT_E_INVALID;
+    }
+  }
+  return B200PT_OK;
 }
 
 // every check of b200pt_set_scene, before its first allocation
@@ -2647,20 +2756,8 @@ int validateScene(b200pt* h, const b200pt_scene_desc& s)
     h->err = msg;
     return B200PT_E_INVALID;
   };
-  for(uint32_t i = 0; i < s.numMaterials; i++)
-  {
-    const b200pt_shade_material& m = s.materials[i];
-    // the 22 texture slots index GltfTextureInfo[] (0 = none, shaders/gltf_scene_io.h.slang:196-219)
-    const uint16_t* slots = &m.pbrBaseColorTexture;
-    for(int k = 0; k < 22; k++)
-      if(slots[k] != 0 && slots[k] >= s.numTextureInfos)
-        return refuse("b200pt_set_scene: material texture slot beyond numTextureInfos");
-    if(m.retroreflectionFactor > 0.0f)
-    {
-      h->err = "b200pt_set_scene: KHR_materials_retroreflection is not built (its lobe lives in nvshaders, external to the reference tree)";
-      return B200PT_E_UNSUPPORTED;
-    }
-  }
+  if(const int rc = validateMaterials(h, "b200pt_set_scene", s.materials, s.numMaterials, s.numTextureInfos))
+    return rc;
   for(uint32_t i = 0; i < s.numTextures; i++)
   {
     const b200pt_texture& t = s.textures[i];
@@ -2677,7 +2774,6 @@ int validateScene(b200pt* h, const b200pt_scene_desc& s)
       return refuse("texture " + std::to_string(i) + " has a sampler enum outside glTF's (wrap " + std::to_string(t.wrapS) + "/" + std::to_string(t.wrapT)
                     + ", filter " + std::to_string(t.magFilter) + "/" + std::to_string(t.minFilter) + ")");
   }
-  bool anyNonOpaque = false;  // as flattenInstances will find it
   for(uint32_t n = 0; n < s.numRenderNodes; n++)
   {
     if(s.renderNodeVisible && !s.renderNodeVisible[n])
@@ -2687,8 +2783,6 @@ int validateScene(b200pt* h, const b200pt_scene_desc& s)
       return refuse("render node references a missing primitive");
     if(node.materialID >= (int)s.numMaterials)
       return refuse("render node references a missing material");
-    if(s.renderPrimitives[node.renderPrimID].triangleCount && !(triFlags(s.materials[(uint32_t)std::max(0, node.materialID)]) & TRI_OPAQUE))
-      anyNonOpaque = true;
   }
   for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
   {
@@ -2697,17 +2791,24 @@ int validateScene(b200pt* h, const b200pt_scene_desc& s)
       if(p.indices[k] >= p.vertexCount)
         return refuse("b200pt_set_scene: index beyond the primitive's vertex count");
   }
-  // the micromaps are linked only into scenes with non-opaque triangles (linkMicromaps)
-  if(anyNonOpaque)
-    for(const auto& po : h->primOmms)
-    {
-      if(po.prim >= s.numRenderPrimitives)
-        return refuse("b200pt_set_scene: opacity micromap linked to a render primitive out of range");
-      const uint32_t nTri = s.renderPrimitives[po.prim].triangleCount;
-      if(po.hasIdx ? po.idx.size() < nTri : (uint64_t)po.base + nTri > h->omms[po.micromap].tris.size())
-        return refuse("b200pt_set_scene: opacity micromap does not cover its primitive's triangles");
-    }
-  return B200PT_OK;
+  return validateMicromaps(h, "b200pt_set_scene", s);
+}
+
+// A path can take more than maxDepth wavefront iterations exactly when k_shade can scatter inside a medium: that is gated on the
+// medium's scatter coefficient (multiscatterColorFactor) of a visible node's material, not on thickness (makeVolumeMedium runs on
+// every transmission event, pathtrace_functions.h.slang:118-140, 605-672)
+bool hasVolumeOf(const b200pt_scene_desc& s)
+{
+  for(uint32_t n = 0; n < s.numRenderNodes; n++)
+  {
+    if(s.renderNodeVisible && !s.renderNodeVisible[n])
+      continue;
+    const b200pt_shade_material& m = s.materials[materialOf(s.renderNodes[n])];
+    if((m.transmissionFactor > 0.0f || m.transmissionTexture || m.diffuseTransmissionFactor > 0.0f || m.diffuseTransmissionTexture)
+       && (m.multiscatterColorFactor[0] > 0.0f || m.multiscatterColorFactor[1] > 0.0f || m.multiscatterColorFactor[2] > 0.0f))
+      return true;
+  }
+  return false;
 }
 
 // which KHR_materials_* features do the scene's materials use (reference: src/scene_feature_detection.cpp)
@@ -2745,10 +2846,12 @@ int uploadTables(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
   const cudaStream_t st = h->stream;
   b.nodesW = A.upload(s.renderNodes, s.numRenderNodes, st);
   b.S.nodes = b.nodesW;
-  b.S.mats = A.upload(s.materials, s.numMaterials, st);
-  b.S.texInfos = A.upload(s.textureInfos, s.numTextureInfos, st);
-  b.S.lights = A.upload(s.lights, s.numLights, st);
+  b.S.mats = b.tableMem.upload(s.materials, s.numMaterials, st);
+  b.S.texInfos = b.tableMem.upload(s.textureInfos, s.numTextureInfos, st);
+  b.S.lights = b.lightMem.upload(s.lights, s.numLights, st);
   b.S.numLights = (int)s.numLights;
+  if(!b.tableMem.ok() || !b.lightMem.ok())
+    return failed(h, b.tableMem.ok() ? b.lightMem : b.tableMem, "scene tables");
   b.primHost.resize(s.numRenderPrimitives);
   std::vector<DevPrim> prims(s.numRenderPrimitives);
   for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
@@ -2841,15 +2944,8 @@ void flattenInstances(const b200pt_scene_desc& s, SceneBuild& b)
       continue;
     const b200pt_render_node&      node = s.renderNodes[n];
     const b200pt_render_primitive& p = s.renderPrimitives[node.renderPrimID];
-    const b200pt_shade_material&   m = s.materials[(uint32_t)std::max(0, node.materialID)];
-    const uint32_t                 flags = triFlags(m);
-    // a path can take more than maxDepth wavefront iterations exactly when k_shade can scatter inside a medium: that
-    // is gated on the medium's scatter coefficient (multiscatterColorFactor), not on thickness (makeVolumeMedium runs on
-    // every transmission event, pathtrace_functions.h.slang:118-140, 605-672)
-    if((m.transmissionFactor > 0.0f || m.transmissionTexture || m.diffuseTransmissionFactor > 0.0f || m.diffuseTransmissionTexture)
-       && (m.multiscatterColorFactor[0] > 0.0f || m.multiscatterColorFactor[1] > 0.0f || m.multiscatterColorFactor[2] > 0.0f))
-      b.hasVolume = true;
-    const float* a = node.objectToWorld;
+    const uint32_t                 flags = triFlags(s.materials[materialOf(node)]);
+    const float*                   a = node.objectToWorld;
     const float  det = a[0] * (a[5] * a[10] - a[9] * a[6]) - a[4] * (a[1] * a[10] - a[9] * a[2]) + a[8] * (a[1] * a[6] - a[5] * a[2]);
     const bool   mirrored = det < 0.0f;
     for(uint32_t t = 0; t < p.triangleCount; t++)
@@ -2986,7 +3082,7 @@ std::vector<std::pair<uint32_t, uint32_t>> levelsOf(const WideBvh& t)
 // Also the trees' views for the refit (b200pt::TreeDev) with their level ranges and box scratch.
 int packTrees(b200pt* h, SceneBuild& b)
 {
-  DeviceArena&       A = b.mem;
+  DeviceArena&       A = b.treeMem;
   const WideBvh &    bvh = b.bvh, &bvhO = b.bvhO, &bvhA = b.bvhA;
   std::vector<float> trisS, packed;
   size_t             offTris = 0, offNodesO = 0, offNodesA = 0, offTrisS = 0;
@@ -3066,8 +3162,7 @@ int packTrees(b200pt* h, SceneBuild& b)
   return B200PT_OK;
 }
 
-// per-triangle attribute records for getHitState (device_scene.cuh: ShadeRec), per render primitive, and the record and material
-// of every triangle slot of the merged tree
+// per-triangle attribute records for getHitState (device_scene.cuh: ShadeRec), per render primitive
 int gatherShadeRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
 {
   DeviceArena&          A = b.mem;
@@ -3116,29 +3211,32 @@ int gatherShadeRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
       }
     }
   }
-  const WideBvh&        bvh = b.bvh;
-  std::vector<uint32_t> idxOfSlot(bvh.numTris, 0u);
-  for(uint32_t k = 0; k < bvh.numTris; k++)
-  {
-    uint32_t gid;
-    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
-    idxOfSlot[k] = recBase[s.renderNodes[b.flat[gid].rnode].renderPrimID] + b.flat[gid].prim;
-  }
-  std::vector<uint32_t> matOfSlot(bvh.numTris, 0u);
-  for(uint32_t k = 0; k < bvh.numTris; k++)
-  {
-    uint32_t gid;
-    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
-    matOfSlot[k] = (uint32_t)std::max(0, s.renderNodes[b.flat[gid].rnode].materialID);
-  }
   b.shadeRecsW = A.upload(recs.data(), recs.size(), h->stream);
   b.S.shadeRecs = b.shadeRecsW;
-  b.S.shadeIdx = A.upload(idxOfSlot.data(), idxOfSlot.size(), h->stream);
-  b.S.matOfSlot = A.upload(matOfSlot.data(), matOfSlot.size(), h->stream);
-  b.S.numMaterials = (int)s.numMaterials;
   for(uint32_t i = 0; i < s.numRenderPrimitives; i++)
     b.primHost[i].recBase = recBase[i];
   return A.ok() ? B200PT_OK : failed(h, A, "shade records");
+}
+
+// the shade record and the material of every triangle slot of the merged tree
+int gatherSlotRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  DeviceArena&          A = b.treeMem;
+  const WideBvh&        bvh = b.bvh;
+  std::vector<uint32_t> idxOfSlot(bvh.numTris, 0u), matOfSlot(bvh.numTris, 0u);
+  for(uint32_t k = 0; k < bvh.numTris; k++)
+  {
+    uint32_t gid;
+    memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
+    const b200pt_render_node& node = s.renderNodes[b.flat[gid].rnode];
+    idxOfSlot[k] = b.primHost[node.renderPrimID].recBase + b.flat[gid].prim;
+    matOfSlot[k] = materialOf(node);
+  }
+  b.S.shadeIdx = A.upload(idxOfSlot.data(), idxOfSlot.size(), h->stream);
+  b.matOfSlotW = A.upload(matOfSlot.data(), matOfSlot.size(), h->stream);
+  b.S.matOfSlot = b.matOfSlotW;
+  b.S.numMaterials = (int)s.numMaterials;
+  return A.ok() ? B200PT_OK : failed(h, A, "slot records");
 }
 
 // alpha-triangle records (device_scene.cuh: AlphaRec), one per non-opaque triangle in bvhA's leaf order
@@ -3146,11 +3244,12 @@ int gatherAlphaRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
 {
   if(!b.anyNonOpaque)
     return B200PT_OK;
-  DeviceArena&          A = b.mem;
+  DeviceArena&          A = b.treeMem;
   const WideBvh &       bvh = b.bvh, &bvhA = b.bvhA;
   const uint32_t        nA = bvhA.numTris;
   std::vector<AlphaRec> recs(nA);
   std::vector<uint32_t> recOfGid(b.flat.size(), 0xFFFFFFFFu);
+  auto                  level0 = [&](int t) { return b.texLevel0[t]; };
   for(uint32_t k = 0; k < nA; k++)
   {
     uint32_t gid;
@@ -3159,45 +3258,8 @@ int gatherAlphaRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
     const FlatTri&                 T = b.flat[gid];
     const b200pt_render_node&      node = s.renderNodes[T.rnode];
     const b200pt_render_primitive& p = s.renderPrimitives[node.renderPrimID];
-    const b200pt_shade_material&   m = s.materials[(uint32_t)std::max(0, node.materialID)];
-    AlphaRec                       r{};
-    r.modeFlags = (uint32_t)m.alphaMode & 3u;
-    r.cutoff = m.alphaCutoff;
-    r.transmission = m.transmissionFactor;
-    const bool     specGloss = m.pbrModel == 1;
-    const uint16_t slot = specGloss ? m.pbrDiffuseTexture : m.pbrBaseColorTexture;
-    r.factor = specGloss ? m.pbrDiffuseFactor[3] : m.pbrBaseColorFactor[3];
-    const uint32_t i0 = p.indices[T.prim * 3], i1 = p.indices[T.prim * 3 + 1], i2 = p.indices[T.prim * 3 + 2];
-    if(slot > 0)
-    {
-      const b200pt_texture_info& ti = s.textureInfos[slot];
-      const float*               uv = ti.texCoord ? p.texCoords[1] : p.texCoords[0];
-      if(uv)
-      {
-        const uint32_t vi[3] = {i0, i1, i2};
-        for(int c = 0; c < 3; c++)
-        {
-          r.uv[c * 2] = uv[vi[c] * 2];
-          r.uv[c * 2 + 1] = uv[vi[c] * 2 + 1];
-        }
-      }
-      if(ti.index >= 0 && (uint32_t)ti.index < s.numTextures)
-      {
-        const DevTex& dt = b.devTex[ti.index];
-        r.lv0 = b.texLevel0[ti.index];
-        r.w0 = dt.w0;
-        r.h0 = dt.h0;
-        r.wrap = ((uint32_t)dt.wrapS & 0xffffu) | ((uint32_t)dt.wrapT << 16);
-        if(dt.magLinear)
-          r.modeFlags |= 4u;
-      }
-    }
-    if(p.colors)
-    {
-      r.modeFlags |= 8u;
-      r.colA = (p.colors[i0] >> 24) | ((p.colors[i1] >> 24) << 8) | ((p.colors[i2] >> 24) << 16);
-    }
-    recs[k] = r;
+    recs[k] = alphaRecOf(s.materials[materialOf(node)], s.textureInfos, b.devTex.data(), s.numTextures, level0, p.texCoords[0], p.texCoords[1],
+                         p.colors, p.indices[T.prim * 3], p.indices[T.prim * 3 + 1], p.indices[T.prim * 3 + 2]);
   }
   std::vector<uint32_t> idxOfSlot(bvh.numTris, 0xFFFFFFFFu);
   for(uint32_t k = 0; k < bvh.numTris; k++)
@@ -3206,7 +3268,8 @@ int gatherAlphaRecs(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
     memcpy(&gid, &bvh.tris[(size_t)k * 12 + 11], 4);
     idxOfSlot[k] = recOfGid[gid];
   }
-  b.S.alphaRecs = A.upload(recs.data(), recs.size(), h->stream);
+  b.alphaRecsW = A.upload(recs.data(), recs.size(), h->stream);
+  b.S.alphaRecs = b.alphaRecsW;
   b.S.alphaIdx = A.upload(idxOfSlot.data(), idxOfSlot.size(), h->stream);
   b.S.alphaBaseS = b.bvhO.numTris;
   return A.ok() ? B200PT_OK : failed(h, A, "alpha records");
@@ -3217,7 +3280,7 @@ int linkMicromaps(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
 {
   if(!b.anyNonOpaque || h->primOmms.empty())
     return B200PT_OK;
-  DeviceArena&          A = b.mem;
+  DeviceArena&          A = b.treeMem;
   const WideBvh &       bvh = b.bvh, &bvhO = b.bvhO, &bvhA = b.bvhA;
   std::vector<uint8_t>  data;
   std::vector<uint32_t> dataBase(h->omms.size());
@@ -3264,30 +3327,77 @@ int linkMicromaps(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
   return A.ok() ? B200PT_OK : failed(h, A, "micromap references");
 }
 
-// hands a built scene to the handle (after the last step that can fail)
-void commitScene(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+// the steps that build the trees and every per-slot table over them into b.treeMem, from the flattened visible triangles
+int buildTreeArena(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
 {
-  h->sceneMem = std::move(b.mem);
-  h->S = b.S;
-  h->numTextureInfos = s.numTextureInfos;
-  h->featureMask = featureMaskOf(s);
-  h->leanShade = (h->featureMask & ~(uint32_t)FEAT_LEAN) == 0;
-  h->primHost = std::move(b.primHost);
-  h->hasVolume = b.hasVolume;
+  flattenInstances(s, b);
+  int rc;
+  if((rc = buildTrees(h, b)) || (rc = packTrees(h, b)) || (rc = gatherSlotRecs(h, s, b)) || (rc = gatherAlphaRecs(h, s, b)) || (rc = linkMicromaps(h, s, b)))
+    return rc;
+  CK(cudaStreamSynchronize(h->stream));
+  return B200PT_OK;
+}
+
+// hands the tree arena of a build to the handle (after the last step that can fail); the previous one is freed
+void commitTrees(b200pt* h, SceneBuild& b)
+{
+  h->treeMem = std::move(b.treeMem);
+  DevScene& S = h->S;
+  S.bvh = b.S.bvh;
+  S.bvhO = b.S.bvhO;
+  S.bvhA = b.S.bvhA;
+  S.hasAlpha = b.S.hasAlpha;
+  S.triMeta = b.S.triMeta;
+  S.triMetaS = b.S.triMetaS;
+  S.matOfSlot = b.S.matOfSlot;
+  S.shadeIdx = b.S.shadeIdx;
+  S.alphaRecs = b.S.alphaRecs;
+  S.alphaIdx = b.S.alphaIdx;
+  S.alphaBaseS = b.S.alphaBaseS;
+  h->dAlphaRecsW = b.alphaRecsW;
+  h->dMatOfSlotW = b.matOfSlotW;
   h->bvhBuildMs = b.bvhBuildMs;
   h->treeBase = b.treeBase;
   h->treeBytes = b.treeBytes;
   for(int t = 0; t < 3; t++)
     h->tree[t] = std::move(b.tree[t]);
-  h->numSceneNodes = s.numRenderNodes;
-  h->dNodesW = b.nodesW;
-  h->dPrimsW = b.S.prims;
-  h->dShadeRecsW = b.shadeRecsW;
   h->ommTriangles = b.ommTriangles;
   h->nodeBytes = b.nodeBytes;
   h->triBytes = b.triBytes;
   h->numNodes = b.bvh.numNodes + (b.anyNonOpaque ? b.bvhO.numNodes + b.bvhA.numNodes : 0u);
   h->numTris = b.bvh.numTris;
+}
+
+// what the materials, the lights and the node visibility decide outside the trees (commitScene and the scene edits)
+void commitFeatures(b200pt* h, const b200pt_scene_desc& s)
+{
+  h->featureMask = featureMaskOf(s);
+  h->leanShade = (h->featureMask & ~(uint32_t)FEAT_LEAN) == 0;
+  h->hasVolume = hasVolumeOf(s);
+}
+
+// hands a built scene to the handle (after the last step that can fail)
+void commitScene(b200pt* h, const b200pt_scene_desc& s, SceneBuild& b)
+{
+  h->sceneMem = std::move(b.mem);
+  h->tableMem = std::move(b.tableMem);
+  h->lightMem = std::move(b.lightMem);
+  h->S = b.S;
+  commitTrees(h, b);
+  h->numTextureInfos = s.numTextureInfos;
+  commitFeatures(h, s);
+  h->primHost = std::move(b.primHost);
+  h->devTex = std::move(b.devTex);
+  h->texLevel0 = std::move(b.texLevel0);
+  h->materials.assign(s.materials, s.materials + s.numMaterials);
+  h->texInfos.assign(s.textureInfos, s.textureInfos + s.numTextureInfos);
+  h->visible.assign(s.numRenderNodes, 1);
+  if(s.renderNodeVisible)
+    h->visible.assign(s.renderNodeVisible, s.renderNodeVisible + s.numRenderNodes);
+  h->numSceneNodes = s.numRenderNodes;
+  h->dNodesW = b.nodesW;
+  h->dPrimsW = b.S.prims;
+  h->dShadeRecsW = b.shadeRecsW;
   h->haveScene = true;
 }
 
@@ -3335,13 +3445,9 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
   SceneBuild b;
   b.S = h->S;  // the environment and the sRGB table
   int rc;
-  if((rc = validateScene(h, *s)) || (rc = uploadTables(h, *s, b)) || (rc = uploadTextures(h, *s, b)))
+  if((rc = validateScene(h, *s)) || (rc = uploadTables(h, *s, b)) || (rc = uploadTextures(h, *s, b)) || (rc = gatherShadeRecs(h, *s, b))
+     || (rc = buildTreeArena(h, *s, b)))
     return rc;
-  flattenInstances(*s, b);
-  if((rc = buildTrees(h, b)) || (rc = packTrees(h, b)) || (rc = gatherShadeRecs(h, *s, b)) || (rc = gatherAlphaRecs(h, *s, b))
-     || (rc = linkMicromaps(h, *s, b)))
-    return rc;
-  CK(cudaStreamSynchronize(h->stream));
   commitScene(h, *s, b);
   setTreeWindow(h);
   return B200PT_OK;
@@ -3602,6 +3708,280 @@ int b200pt_update_node_matrices(b200pt_t* h, const float* local_matrices)
   }
   CK(cudaGetLastError());
   return refitTrees(h);
+}
+
+}  // extern "C"
+namespace {
+
+// ---- scene edits (b200pt_update_materials, b200pt_update_node_materials, b200pt_set_node_visibility) -------------------------------
+// An edited handle renders what a fresh b200pt_set_scene of the edited description renders.  Two paths:
+//   in place  the visible set is unchanged and no visible triangle changes TRI_OPAQUE: the tables are replaced and k_retag_tris /
+//             k_gather_alpha rewrite what the materials decide in the trees' triangle records and the alpha records;
+//   rebuild   otherwise (shadow-tree membership, the alpha records and the micromap links follow TRI_OPAQUE): the tree arena is
+//             built again by b200pt_set_scene's own steps, from the primitives' CURRENT vertices and the nodes' CURRENT transforms,
+//             so an animated pose survives.  The per-primitive shade records are not touched (they may hold that pose).
+
+// the scene the handle holds, as a scene description: the render nodes as the device has them (transforms and material ids may
+// have moved since b200pt_set_scene), the host copies of the tables and the visibility; loadGeometry adds the primitives' current
+// vertex data
+struct CurrentScene
+{
+  std::vector<b200pt_render_node>      nodes;
+  std::vector<b200pt_render_primitive> prims;
+  std::vector<std::vector<uint32_t>>   idx, col;
+  std::vector<std::vector<float>>      pos, uv0, uv1;
+  b200pt_scene_desc                    desc{};
+};
+
+int loadCurrentScene(b200pt* h, CurrentScene& c)
+{
+  c.nodes.resize(h->numSceneNodes);
+  CK(cudaMemcpy(c.nodes.data(), h->dNodesW, c.nodes.size() * sizeof(b200pt_render_node), cudaMemcpyDeviceToHost));
+  c.prims.assign(h->primHost.size(), b200pt_render_primitive{});
+  for(size_t i = 0; i < c.prims.size(); i++)
+  {
+    c.prims[i].triangleCount = h->primHost[i].triCount;
+    c.prims[i].vertexCount = h->primHost[i].vertexCount;
+  }
+  b200pt_scene_desc& d = c.desc;
+  d.renderNodes = c.nodes.data();
+  d.numRenderNodes = h->numSceneNodes;
+  d.renderNodeVisible = h->visible.data();
+  d.renderPrimitives = c.prims.data();
+  d.numRenderPrimitives = (uint32_t)c.prims.size();
+  d.materials = h->materials.data();
+  d.numMaterials = (uint32_t)h->materials.size();
+  d.textureInfos = h->texInfos.data();
+  d.numTextureInfos = (uint32_t)h->texInfos.size();
+  d.numTextures = (uint32_t)h->S.numTextures;
+  d.numLights = (uint32_t)h->S.numLights;
+  return B200PT_OK;
+}
+
+// the vertex data a tree rebuild reads: indices, positions, texture coordinates and colours of every primitive
+int loadGeometry(b200pt* h, CurrentScene& c)
+{
+  const size_t n = c.prims.size();
+  c.idx.resize(n), c.col.resize(n), c.pos.resize(n), c.uv0.resize(n), c.uv1.resize(n);
+  for(size_t i = 0; i < n; i++)
+  {
+    const b200pt::PrimHost& P = h->primHost[i];
+    b200pt_render_primitive& p = c.prims[i];
+    const size_t            nv = P.vertexCount;
+    auto fetch = [&](auto& dst, const auto* src, size_t count) -> const typename std::decay_t<decltype(dst)>::value_type* {
+      if(!src)
+        return nullptr;
+      dst.resize(count);
+      return cudaMemcpy(dst.data(), src, count * sizeof(dst[0]), cudaMemcpyDeviceToHost) == cudaSuccess ? dst.data() : nullptr;
+    };
+    p.indices = fetch(c.idx[i], P.d.idx, (size_t)P.triCount * 3);
+    p.positions = fetch(c.pos[i], P.d.pos, nv * 3);
+    p.texCoords[0] = fetch(c.uv0[i], P.d.uv0, nv * 2);
+    p.texCoords[1] = fetch(c.uv1[i], P.d.uv1, nv * 2);
+    p.colors = fetch(c.col[i], P.d.col, nv);
+    if(!p.indices || !p.positions || (P.d.uv0 && !p.texCoords[0]) || (P.d.uv1 && !p.texCoords[1]) || (P.d.col && !p.colors))
+    {
+      cudaGetLastError();
+      h->err = "scene edit: reading the primitives' vertex data back failed";
+      return B200PT_E_CUDA;
+    }
+  }
+  return B200PT_OK;
+}
+
+// Applies an edit whose every argument has been checked: `next` is the current scene `cur` with the edit applied.  newTables:
+// next's materials / texture infos replace the tables; newIds: the render nodes' material ids (`next`'s) are written to the device
+// nodes and the hierarchy's mappings.  The replacements are built before anything is swapped, so a failed allocation leaves the
+// scene as it was.
+int applySceneEdit(b200pt* h, const char* who, CurrentScene& cur, const b200pt_scene_desc& next, bool newTables, const int32_t* newIds)
+{
+  const b200pt_scene_desc& old = cur.desc;
+  bool                     rebuild = false;
+  for(uint32_t n = 0; n < old.numRenderNodes && !rebuild; n++)
+  {
+    const bool v = next.renderNodeVisible[n] != 0;
+    rebuild = v != (old.renderNodeVisible[n] != 0);
+    if(v && !rebuild && old.renderPrimitives[next.renderNodes[n].renderPrimID].triangleCount)
+      rebuild = ((triFlags(old.materials[materialOf(old.renderNodes[n])]) ^ triFlags(next.materials[materialOf(next.renderNodes[n])])) & TRI_OPAQUE) != 0;
+  }
+  if(rebuild)
+    if(const int rc = validateMicromaps(h, who, next))
+      return rc;
+  const cudaStream_t st = h->stream;
+  DeviceArena        tables;
+  const b200pt_shade_material* dMats = h->S.mats;
+  const b200pt_texture_info*   dTexInfos = h->S.texInfos;
+  if(newTables)
+  {
+    dMats = tables.upload(next.materials, next.numMaterials, st);
+    dTexInfos = tables.upload(next.textureInfos, next.numTextureInfos, st);
+    if(!tables.ok())
+      return failed(h, tables, who);
+  }
+  SceneBuild b;
+  if(rebuild)
+  {
+    b.S = h->S;
+    b.primHost = h->primHost;
+    b.devTex = h->devTex;
+    b.texLevel0 = h->texLevel0;
+    int rc;
+    if((rc = loadGeometry(h, cur)) || (rc = buildTreeArena(h, next, b)))
+      return rc;
+  }
+  // nothing below allocates
+  if(newIds && next.numRenderNodes)
+  {
+    CK(cudaMemcpy2DAsync(reinterpret_cast<char*>(h->dNodesW) + offsetof(b200pt_render_node, materialID), sizeof(b200pt_render_node), newIds, sizeof(int32_t),
+                         sizeof(int32_t), next.numRenderNodes, cudaMemcpyHostToDevice, st));
+    // (or the next b200pt_update_node_matrices would write the old ids back)
+    if(h->graph.dMappings)
+      CK(cudaMemcpy2DAsync(reinterpret_cast<char*>(h->graph.dMappings) + offsetof(RenderNodeMapping, materialID), sizeof(RenderNodeMapping), newIds,
+                           sizeof(int32_t), sizeof(int32_t), next.numRenderNodes, cudaMemcpyHostToDevice, st));
+  }
+  if(newTables)
+  {
+    h->tableMem = std::move(tables);
+    h->S.mats = dMats;
+    h->S.texInfos = dTexInfos;
+    h->materials.assign(next.materials, next.materials + next.numMaterials);
+    h->texInfos.assign(next.textureInfos, next.textureInfos + next.numTextureInfos);
+    h->numTextureInfos = next.numTextureInfos;
+  }
+  h->visible.assign(next.renderNodeVisible, next.renderNodeVisible + next.numRenderNodes);
+  commitFeatures(h, next);
+  if(rebuild)
+  {
+    commitTrees(h, b);
+    setTreeWindow(h);
+  }
+  else
+  {
+    const DevScene& S = h->S;
+    for(int t = 0; t < 2; t++)
+    {
+      const b200pt::TreeDev& T = h->tree[t];
+      if(T.nodes && T.numTriSlots)
+      {
+        k_retag_tris<<<gridFor(h, 4), 256, 0, st>>>(T.tris, T.meta, t == 0 ? h->dMatOfSlotW : nullptr, T.numTriSlots, h->dNodesW, S.mats);
+        h->kernelLaunches++;
+      }
+    }
+    if(h->dAlphaRecsW)
+    {
+      k_gather_alpha<<<gridFor(h, 4), 256, 0, st>>>(h->dAlphaRecsW, S.triMetaS, S.alphaBaseS, h->tree[1].numTriSlots - S.alphaBaseS, S);
+      h->kernelLaunches++;
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(st));
+  return B200PT_OK;
+}
+
+}  // namespace
+extern "C" {
+
+int b200pt_update_materials(b200pt_t* h, const b200pt_shade_material* materials, uint32_t num_materials, const b200pt_texture_info* texture_infos,
+                            uint32_t num_texture_infos)
+{
+  const char* who = "b200pt_update_materials";
+  if(!h || !h->haveScene || !materials || num_materials != h->materials.size() || (num_texture_infos && !texture_infos))
+  {
+    if(h)
+      h->err = std::string(who) + ": needs a scene and a material table of the scene's material count";
+    return B200PT_E_INVALID;
+  }
+  int rc;
+  if((rc = enter(h, true)) || (rc = validateMaterials(h, who, materials, num_materials, num_texture_infos)))
+    return rc;
+  CurrentScene cur;
+  if((rc = loadCurrentScene(h, cur)))
+    return rc;
+  b200pt_scene_desc next = cur.desc;
+  next.materials = materials;
+  next.textureInfos = texture_infos;
+  next.numTextureInfos = num_texture_infos;
+  return applySceneEdit(h, who, cur, next, true, nullptr);
+}
+
+int b200pt_update_node_materials(b200pt_t* h, const int32_t* material_ids, uint32_t num_nodes)
+{
+  const char* who = "b200pt_update_node_materials";
+  if(!h || !h->haveScene || (num_nodes && !material_ids) || num_nodes != h->numSceneNodes)
+  {
+    if(h)
+      h->err = std::string(who) + ": needs a scene and one material id per render node";
+    return B200PT_E_INVALID;
+  }
+  for(uint32_t n = 0; n < num_nodes; n++)
+    if(material_ids[n] >= (int32_t)h->materials.size())
+    {
+      h->err = std::string(who) + ": render node references a missing material";
+      return B200PT_E_INVALID;
+    }
+  int rc;
+  CurrentScene cur;
+  if((rc = enter(h, true)) || (rc = loadCurrentScene(h, cur)))
+    return rc;
+  std::vector<b200pt_render_node> nodes = cur.nodes;
+  for(uint32_t n = 0; n < num_nodes; n++)
+    nodes[n].materialID = material_ids[n];
+  b200pt_scene_desc next = cur.desc;
+  next.renderNodes = nodes.data();
+  return applySceneEdit(h, who, cur, next, false, material_ids);
+}
+
+int b200pt_set_node_visibility(b200pt_t* h, const uint8_t* visible, uint32_t num_nodes)
+{
+  const char* who = "b200pt_set_node_visibility";
+  if(!h || !h->haveScene || (num_nodes && !visible) || num_nodes != h->numSceneNodes)
+  {
+    if(h)
+      h->err = std::string(who) + ": needs a scene and one flag per render node";
+    return B200PT_E_INVALID;
+  }
+  int rc;
+  CurrentScene cur;
+  if((rc = enter(h, true)) || (rc = loadCurrentScene(h, cur)))
+    return rc;
+  std::vector<uint8_t> vis(num_nodes);
+  for(uint32_t n = 0; n < num_nodes; n++)
+  {
+    vis[n] = visible[n] ? 1 : 0;
+    // b200pt_set_scene checks visible nodes only: one that becomes visible is checked here
+    const b200pt_render_node& node = cur.nodes[n];
+    if(vis[n] && (node.renderPrimID < 0 || (uint32_t)node.renderPrimID >= cur.desc.numRenderPrimitives || node.materialID >= (int)cur.desc.numMaterials))
+    {
+      h->err = std::string(who) + ": a visible render node references a missing primitive or material";
+      return B200PT_E_INVALID;
+    }
+  }
+  b200pt_scene_desc next = cur.desc;
+  next.renderNodeVisible = vis.data();
+  return applySceneEdit(h, who, cur, next, false, nullptr);
+}
+
+int b200pt_update_lights(b200pt_t* h, const b200pt_light* lights, uint32_t num_lights)
+{
+  if(!h || !h->haveScene || (num_lights && !lights))
+  {
+    if(h)
+      h->err = "b200pt_update_lights: needs a scene and the light array";
+    return B200PT_E_INVALID;
+  }
+  if(const int rc = enter(h, true))
+    return rc;
+  DeviceArena         L;
+  const b200pt_light* dLights = L.upload(lights, num_lights, h->stream);
+  if(!L.ok())
+    return failed(h, L, "b200pt_update_lights");
+  CK(cudaStreamSynchronize(h->stream));
+  h->lightMem = std::move(L);
+  h->S.lights = dLights;
+  h->S.numLights = (int)num_lights;
+  h->featureMask = (h->featureMask & ~(uint32_t)FEAT_LIGHTS) | (num_lights ? (uint32_t)FEAT_LIGHTS : 0u);
+  h->leanShade = (h->featureMask & ~(uint32_t)FEAT_LEAN) == 0;
+  return B200PT_OK;
 }
 
 int b200pt_set_animation(b200pt_t* h, const b200pt_morph_task* morphs, uint32_t num_morphs, const b200pt_skin_task* skins, uint32_t num_skins)

@@ -73,6 +73,69 @@ struct ShadeRec
 };
 static_assert(sizeof(ShadeRec) == 192, "ShadeRec is twelve 16-byte loads");
 
+// ---- per-triangle derivations from a render node's material, shared by b200pt_set_scene (host) and the scene-edit kernels ----
+
+// material index of a render node (-1 = material 0)
+PT_HD uint32_t materialOf(const b200pt_render_node& node) { return node.materialID > 0 ? (uint32_t)node.materialID : 0u; }
+
+// the instance flags of a material's triangles (getInstanceFlag, src/gltf_scene_rtx.cpp:271-295)
+PT_HD uint32_t triFlags(const b200pt_shade_material& m)
+{
+  uint32_t flags = 0;
+  if(m.transmissionFactor == 0.0f && m.alphaMode == 0 && m.diffuseTransmissionFactor == 0.0f)
+    flags |= TRI_OPAQUE;
+  if(m.doubleSided == 1 || m.thicknessFactor > 0.0f || m.transmissionFactor > 0.0f)
+    flags |= TRI_NOCULL;
+  return flags;
+}
+
+// The alpha-test record of one non-opaque triangle with vertex indices i0..i2 of a primitive (uv0 / uv1 / colors may be null).
+// `textures` are the DevTex records and level0(t) the level-0 texels of texture t (the host keeps them in its own table, the
+// device reads them through the record's level offsets).
+#pragma nv_exec_check_disable
+template <class Level0>
+PT_HD AlphaRec alphaRecOf(const b200pt_shade_material& m, const b200pt_texture_info* texInfos, const DevTex* textures, uint32_t numTextures,
+                          Level0 level0, const float* uv0, const float* uv1, const uint32_t* colors, uint32_t i0, uint32_t i1, uint32_t i2)
+{
+  AlphaRec r{};
+  r.modeFlags = (uint32_t)m.alphaMode & 3u;
+  r.cutoff = m.alphaCutoff;
+  r.transmission = m.transmissionFactor;
+  const bool     specGloss = m.pbrModel == 1;
+  const uint16_t slot = specGloss ? m.pbrDiffuseTexture : m.pbrBaseColorTexture;
+  r.factor = specGloss ? m.pbrDiffuseFactor[3] : m.pbrBaseColorFactor[3];
+  if(slot > 0)
+  {
+    const b200pt_texture_info& ti = texInfos[slot];
+    const float*               uv = ti.texCoord ? uv1 : uv0;
+    if(uv)
+    {
+      const uint32_t vi[3] = {i0, i1, i2};
+      for(int c = 0; c < 3; c++)
+      {
+        r.uv[c * 2] = uv[vi[c] * 2];
+        r.uv[c * 2 + 1] = uv[vi[c] * 2 + 1];
+      }
+    }
+    if(ti.index >= 0 && (uint32_t)ti.index < numTextures)
+    {
+      const DevTex& dt = textures[ti.index];
+      r.lv0 = level0(ti.index);
+      r.w0 = dt.w0;
+      r.h0 = dt.h0;
+      r.wrap = ((uint32_t)dt.wrapS & 0xffffu) | ((uint32_t)dt.wrapT << 16);
+      if(dt.magLinear)
+        r.modeFlags |= 4u;
+    }
+  }
+  if(colors)
+  {
+    r.modeFlags |= 8u;
+    r.colA = (colors[i0] >> 24) | ((colors[i1] >> 24) << 8) | ((colors[i2] >> 24) << 16);
+  }
+  return r;
+}
+
 struct DevScene
 {
   const b200pt_render_node*    nodes;

@@ -152,6 +152,32 @@ class PathTracer:
             arr[i].renderPrimID = rn["renderPrimID"]
         self._ck(self._L.b200pt_update_transforms(self._h, arr, n), "b200pt_update_transforms")
 
+    # -- scene edits (GltfRenderer::updateSceneChanges): the handle then renders what onSceneInvalidated of the edited scene would --
+    def update_materials(self, resources):
+        """the materials / texture infos of resources.scene changed (same material count, same texture images): b200pt_update_materials"""
+        scn = resources.scene
+        mats = (abi.ShadeMaterial * max(len(scn.materials), 1))(*scn.materials)
+        tis = (abi.TextureInfo * max(len(scn.texture_infos), 1))(*scn.texture_infos)
+        self._ck(self._L.b200pt_update_materials(self._h, mats, len(scn.materials), tis, len(scn.texture_infos)), "b200pt_update_materials")
+
+    def update_node_materials(self, resources):
+        """the render nodes' materialIDs of resources.scene changed (a material variant switch): b200pt_update_node_materials"""
+        ids = np.ascontiguousarray([rn["materialID"] for rn in resources.scene.render_nodes] or [0], np.int32)
+        self._ck(self._L.b200pt_update_node_materials(self._h, ids.ctypes.data_as(C.POINTER(C.c_int32)), len(resources.scene.render_nodes)),
+                 "b200pt_update_node_materials")
+
+    def update_lights(self, resources):
+        """the lights of resources.scene changed (their count too): b200pt_update_lights"""
+        lights = resources.scene.lights
+        arr = (abi.Light * max(len(lights), 1))(*lights)
+        self._ck(self._L.b200pt_update_lights(self._h, arr, len(lights)), "b200pt_update_lights")
+
+    def set_node_visibility(self, resources):
+        """the render nodes' visibility of resources.scene changed: b200pt_set_node_visibility"""
+        vis = np.ascontiguousarray([1 if rn.get("visible", True) else 0 for rn in resources.scene.render_nodes] or [0], np.uint8)
+        self._ck(self._L.b200pt_set_node_visibility(self._h, vis.ctypes.data_as(C.POINTER(C.c_uint8)), len(resources.scene.render_nodes)),
+                 "b200pt_set_node_visibility")
+
     def set_animation(self, morph_tasks=(), skin_tasks=()):
         """SceneAnimationVk::createAnimationResources analogue (b200pt_set_animation): uploads the static inputs of the morph /
         skin tasks (vk_gltf_renderer_b200.animation.MorphTask / SkinTask) of the current scene."""

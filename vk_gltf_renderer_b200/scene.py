@@ -62,6 +62,12 @@ class Scene:
         self.graph = None             # dict(parents i32[N], locals f64[N,4,4], render_nodes [(nodeID, skinID, instLocal f64[4,4])], skins [dict(joints, ibm)], mesh_weights {mesh: f32[T]})
         self.morph_prims = {}         # renderPrimID -> dict(mesh, position_deltas f32[T,V,3], normal_deltas | None, tangent_deltas | None)
         self.skin_prims = {}          # renderPrimID -> dict(joints i32[V,4], weights f32[V,4])
+        # KHR_materials_variants: the root's variant names; a loaded render node carries its primitive's mappings
+        # ("variantMaterials": {variant: material}) and its own material ("defaultMaterial")
+        self.variants = []
+        # KHR_node_visibility: every glTF node's own flag (a loaded scene); a render node is visible when its node and every
+        # ancestor are (Scene::traverseSceneWithVisibility)
+        self.node_visible = None
         self._keep = []
 
     # -- bounds (reference: Scene::getSceneBounds, gltf_scene.cpp:2303-2336, from transformed vertices)
@@ -75,6 +81,33 @@ class Scene:
             lo = np.minimum(lo, w.min(0))
             hi = np.maximum(hi, w.max(0))
         return lo, hi
+
+    def set_variant(self, variant):
+        """Scene::setCurrentVariant: every render node takes its primitive's material for `variant` (an index into
+        self.variants), or its own material where the primitive maps none; None restores the own materials.  Push the
+        result with PathTracer.update_node_materials."""
+        for rn in self.render_nodes:
+            if "defaultMaterial" in rn:
+                rn["materialID"] = rn["variantMaterials"].get(variant, rn["defaultMaterial"])
+
+    def set_node_visible(self, node, visible):
+        """KHR_node_visibility of glTF node `node`; the render nodes below it follow (an invisible node hides its whole
+        subtree).  Push the result with PathTracer.set_node_visibility."""
+        if self.node_visible is None:
+            raise ValueError("set_node_visible needs a scene loaded from glTF (its node graph)")
+        self.node_visible[node] = bool(visible)
+        self._apply_visibility()
+
+    def _apply_visibility(self):
+        parents = self.graph["parents"]
+        memo = {}
+
+        def shown(n):
+            if n not in memo:
+                memo[n] = self.node_visible[n] and (parents[n] < 0 or shown(int(parents[n])))
+            return memo[n]
+        for rn, (nid, _, _) in zip(self.render_nodes, self.graph["render_nodes"]):
+            rn["visible"] = shown(nid)
 
     def num_triangles(self):
         return sum(len(self.render_prims[rn["renderPrimID"]]["indices"]) for rn in self.render_nodes
@@ -814,7 +847,6 @@ def load_gltf(path):
                 L.angularSizeOrInvRange = 1.0 / rng if rng > 0 else 0.0
             scn.lights.append(L)
         if node.get("mesh", -1) > -1:
-            visible = node.get("extensions", {}).get("KHR_node_visibility", {}).get("visible", True)
             inst = node.get("extensions", {}).get("EXT_mesh_gpu_instancing")
             locals_ = [np.eye(4)]
             if inst:
@@ -829,14 +861,20 @@ def load_gltf(path):
             for p in j["meshes"][node["mesh"]]["primitives"]:
                 if p.get("mode", 4) != 4:
                     continue
+                variant_materials = {v: mp["material"] for mp in p.get("extensions", {}).get("KHR_materials_variants", {}).get("mappings", [])
+                                     for v in mp.get("variants", []) if "material" in mp}
                 for lm in locals_:
-                    scn.add_node(prim_map[prim_key(p)], p.get("material", -1), world @ lm, visible)
+                    scn.add_node(prim_map[prim_key(p)], p.get("material", -1), world @ lm)
+                    scn.render_nodes[-1].update(defaultMaterial=p.get("material", -1), variantMaterials=variant_materials)
                     scn.graph["render_nodes"].append((nid, node.get("skin", -1), np.asarray(lm, np.float64)))   # RenderNode::refNodeID / skinID
         for c in node.get("children", []):
             visit(c, world)
 
     for root in j.get("scenes", [{"nodes": list(range(len(nodes)))}])[scene_id]["nodes"]:
         visit(root, np.eye(4))
+    scn.variants = [v.get("name", "") for v in j.get("extensions", {}).get("KHR_materials_variants", {}).get("variants", [])]
+    scn.node_visible = [bool(n.get("extensions", {}).get("KHR_node_visibility", {}).get("visible", True)) for n in nodes]
+    scn._apply_visibility()
 
     # ---- camera (Scene::handleCameraTraversal) ----
     if cam_found:
