@@ -268,9 +268,9 @@ __device__ __forceinline__ uint32_t fetchWork(bool need, uint32_t* workCounter, 
 // The persistent-warp loop of the walk kernels, over the `count` paths of queue q.  Per lane: path (-1 needs work, -2
 // exhausted) and a resumable traversal; finished lanes are handled in the converged part of the loop, never inside the
 // traversal loop.  start(T, path) begins the walk of a fetched path; finish(T, cand, path) writes a finished walk out and
-// returns whether the lane is free (false: it started T again on the same path).  OMM, MODE and omm are those of
+// returns whether the lane is free (false: it started T again on the same path).  OMM, CAPS, MODE and omm are those of
 // TravState::step (MODE 1: closest-hit walk, 2: shadow walk); a continuation round (cont) does not count its rays again.
-template <bool OMM, int MODE, class Start, class Finish>
+template <bool OMM, bool CAPS, int MODE, class Start, class Finish>
 __device__ __forceinline__ void walkQueue(const uint32_t* __restrict__ q, uint32_t count, uint32_t* workCounter, const BvhView& omm, DevStats* stats, bool cont,
                                           Start start, Finish finish)
 {
@@ -326,7 +326,7 @@ __device__ __forceinline__ void walkQueue(const uint32_t* __restrict__ q, uint32
       }
 #endif
       if(path >= 0 && !travDone)
-        travDone = T.step<kCand, false, OMM, MODE>(stack, kPostponeShift, cand, kWalkBlock, omm.ommRef, omm.ommData);
+        travDone = T.step<kCand, false, OMM, MODE, CAPS>(stack, kPostponeShift, cand, kWalkBlock, omm.ommRef, omm.ommData, omm.capRef, omm.capBits);
       if(__popc(__ballot_sync(0xffffffffu, path >= 0 && !travDone)) < kRefillThreshold)
         break;
     }
@@ -347,7 +347,7 @@ enum : int
   TRACE_CONT = 1,
   TRACE_TMIN = 2,
 };
-template <bool OMM>
+template <bool OMM, bool CAPS>
 __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_trace(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
                                                                       uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
 {
@@ -384,7 +384,7 @@ __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_trace(PathState 
     }
     return true;
   };
-  walkQueue<OMM, 1>(q, *cntIn, workCounter, S.bvh, stats, cont, start, finish);
+  walkQueue<OMM, CAPS, 1>(q, *cntIn, workCounter, S.bvh, stats, cont, start, finish);
 }
 
 // Any-hit part of IRaytracer::Trace (SHADOW = false) and IRaytracer::TraceShadow (SHADOW = true): the candidates
@@ -1129,7 +1129,7 @@ __device__ void finishPost(const PathState& P, const DevScene& S, const FramePar
 // nearest non-opaque candidates are written out for k_alpha<true>.  Same persistent-warp scheme as k_trace.
 // candInfo.x of a shadow ray that an opaque occluder ended (raytracer_interface.h.slang:181-184)
 constexpr uint32_t kShadowOccluded = 0x80000000u;
-template <bool OMM>
+template <bool OMM, bool CAPS>
 __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_shadow(PathState P, DevScene S, const uint32_t* __restrict__ q, const uint32_t* __restrict__ cntIn,
                                                                        uint32_t* workCounter, uint32_t* qAlpha, uint32_t* cntAlpha, DevStats* stats, int mode)
 {
@@ -1180,8 +1180,8 @@ __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_shadow(PathState
       queuePush(qAlpha, cntAlpha, (uint32_t)path);
     return true;
   };
-  // (only the non-opaque triangles of phase 1 consult the micromaps)
-  walkQueue<OMM, 2>(q, *cntIn, workCounter, S.bvhA, stats, cont, start, finish);
+  // (only the non-opaque triangles of phase 1 consult the micromaps and the caps)
+  walkQueue<OMM, CAPS, 2>(q, *cntIn, workCounter, S.bvhA, stats, cont, start, finish);
 }
 
 // ---- material-sorted shade queue (north star: "material-sorted shade queues to tame divergence") -------------------------
@@ -1628,6 +1628,28 @@ __global__ void __launch_bounds__(256) k_gather_alpha(AlphaRec* recs, const uint
   }
 }
 
+// the alpha caps of the alpha records (alpha_caps.cuh), one thread per (record, grid cell of kCapLevel): the cap micro-triangles of
+// record r are OR-ed into bits[r * kCapWords ...] (zeroed by the caller); shadowOk[r]: the record's material may cap a shadow ray
+#pragma nv_exec_check_disable
+__global__ void __launch_bounds__(256) k_cap_bake(const AlphaRec* __restrict__ recs, uint32_t n, uint32_t* bits, uint8_t* shadowOk)
+{
+  constexpr uint32_t cells = 2u * kCapMicro;
+  const uint64_t     total = (uint64_t)n * cells, stride = (uint64_t)gridDim.x * blockDim.x;
+  for(uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride)
+  {
+    const uint32_t rec = (uint32_t)(i / cells), k = (uint32_t)(i % cells);
+    const AlphaRec r = loadAlphaRec(recs + rec);
+    if(k == 0)
+      shadowOk[rec] = r.transmission <= 0.01f ? 1 : 0;
+    const int tpr = (r.w0 + 3) >> 2;
+    auto      alpha8 = [&](int x, int y) { return (int)__ldg(r.lv0 + (((y >> 2) * tpr + (x >> 2)) << 4) + ((y & 3) << 2) + (x & 3)).w; };
+    auto      wrap = [](int i, int m, int mode) { return wrapFast(i, m, mode); };
+    uint32_t  idx;
+    if(capBakeCell(k, r.uv, r.w0, r.h0, r.wrap, r.factor, r.cutoff, r.modeFlags, r.colA, r.lv0 != nullptr, alpha8, wrap, idx))
+      atomicOr(&bits[(size_t)rec * kCapWords + (idx >> 5)], 1u << (idx & 31u));
+  }
+}
+
 // ---- ray-level API (parity tests / traversal micro-benchmark): the rays run through the PRODUCTION kernels
 // (k_trace / k_shadow -> k_alpha -> continuation round -> k_alpha) on a scratch path pool -------------------------
 __global__ void __launch_bounds__(256) k_rays_load(PathState P, const float4* __restrict__ rays, uint32_t n, const uint32_t* __restrict__ seeds, uint32_t* q, uint32_t* cnt,
@@ -1904,6 +1926,7 @@ struct b200pt
   std::vector<OmmHost>     omms;
   std::vector<PrimOmmHost> primOmms;
   uint32_t                 ommTriangles = 0;  // non-opaque triangles of the scene that got a micromap / special state
+  DeviceArena              capMem;            // the alpha caps (alpha_caps.cuh), baked again after every change of the alpha records
   DevScene            S{};
   bool                haveScene = false;
   uint32_t            numTextureInfos = 0;  // S.texInfos entries (host copy of the count, for argument checks)
@@ -2219,6 +2242,7 @@ void freeScene(b200pt* h)
   h->anim = b200pt::Animation{};
   h->graph = b200pt::Hierarchy{};
   h->treeMem.release();
+  h->capMem.release();
   h->tableMem.release();
   h->lightMem.release();
   h->sceneMem.release();
@@ -2458,9 +2482,11 @@ void launchWalk(const Launcher& ctx, int shadow, const PathState& P, const uint3
 {
   const b200pt*   h = ctx.h;
   const DevScene& S = h->S;
-  // the walk kernels have an instantiation for scenes with opacity micromaps (omm.cuh) and one without the lookup
-  const bool  omm = S.bvh.ommRef != nullptr;
-  const auto  walk = shadow ? (omm ? k_shadow<true> : k_shadow<false>) : (omm ? k_trace<true> : k_trace<false>);
+  // the walk kernels have an instantiation for scenes with opacity micromaps (omm.cuh), one for scenes with alpha caps (alpha_caps.cuh)
+  // and one without either lookup
+  const bool  omm = S.bvh.ommRef != nullptr, caps = S.bvh.capRef != nullptr;
+  const auto  walk = shadow ? (omm ? k_shadow<true, false> : caps ? k_shadow<false, true> : k_shadow<false, false>)
+                            : (omm ? k_trace<true, false> : caps ? k_trace<false, true> : k_trace<false, false>);
   const auto  alpha = shadow ? k_alpha<true> : k_alpha<false>;
   const Stage stage = shadow ? kStageShadow : kStageTrace;
   const int   gA = gridFor(h, 8), gW = gridFor(h, kWalkCtasPerSM), R = h->contRounds;
@@ -3117,6 +3143,8 @@ int packTrees(b200pt* h, SceneBuild& b)
   S.bvh.tris = reinterpret_cast<const float4*>(dPacked + offTris);
   S.bvh.ommRef = nullptr;
   S.bvh.ommData = nullptr;
+  S.bvh.capRef = nullptr;
+  S.bvh.capBits = nullptr;
   S.hasAlpha = b.anyNonOpaque ? 1 : 0;
   S.triMeta = reinterpret_cast<const uint2*>(dMeta);
   S.bvhO = S.bvh;
@@ -3428,6 +3456,102 @@ void setTreeWindow(b200pt* h)
   }
 }
 
+// The alpha caps (alpha_caps.cuh) of the handle's scene, baked from its alpha records into h->capMem: the reference words of the
+// closest-hit tree and of the shadow rays' triangle array, and the bit maps of the triangles that have both cap and non-cap
+// micro-triangles.  Called after every change of the alpha records (b200pt_set_scene, a scene edit that changed an alpha input, a
+// rebuild).  Scenes with opacity micromaps or without non-opaque triangles get none, and so does every scene while
+// B200PT_ALPHA_CAPS=0 (caps change no result: the switch lets the tests compare walks with and without them).  The records are baked
+// kChunk at a time, so the unpacked maps in flight stay at kChunk x 128 B on the device and on the host whatever the scene's size.
+// Returns an error code with h->err set on a failure; the handle is then left without caps.
+int bakeAlphaCaps(b200pt* h)
+{
+  DevScene& S = h->S;
+  for(BvhView* v : {&S.bvh, &S.bvhO, &S.bvhA})
+    v->capRef = v->capBits = nullptr;
+  h->capMem.release();
+  const char* e = getenv("B200PT_ALPHA_CAPS");
+  if(!S.hasAlpha || S.bvh.ommRef || !h->dAlphaRecsW || (e && atoi(e) == 0))
+    return B200PT_OK;
+  constexpr uint32_t kChunk = 1u << 16;
+  const cudaStream_t st = h->stream;
+  const uint32_t     nC = h->tree[0].numTriSlots, nS = h->tree[1].numTriSlots, base = S.alphaBaseS, nA = nS - base;
+  DeviceArena        scratch;
+  uint32_t* const    dBits = scratch.alloc<uint32_t>((size_t)std::min(nA, kChunk) * kCapWords);
+  uint8_t* const     dShadowOk = scratch.alloc<uint8_t>(std::min(nA, kChunk));
+  if(!scratch.ok())
+    return failed(h, scratch, "alpha caps");
+  // per record: no cap, all caps, or its map appended to the packed bits
+  std::vector<uint32_t> refOfRec(nA, kCapNone), packed, bits((size_t)std::min(nA, kChunk) * kCapWords);
+  std::vector<uint8_t>  shadowOk(nA);
+  bool                  any = false;
+  for(uint32_t r0 = 0; r0 < nA; r0 += kChunk)
+  {
+    const uint32_t n = std::min(kChunk, nA - r0);
+    CK(cudaMemsetAsync(dBits, 0, (size_t)n * kCapWords * sizeof(uint32_t), st));
+    k_cap_bake<<<gridFor(h, 8), 256, 0, st>>>(S.alphaRecs + r0, n, dBits, dShadowOk);
+    h->kernelLaunches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(bits.data(), dBits, (size_t)n * kCapWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(shadowOk.data() + r0, dShadowOk, n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for(uint32_t r = 0; r < n; r++)
+    {
+      const uint32_t* m = &bits[(size_t)r * kCapWords];
+      uint32_t        caps = 0;
+      for(uint32_t w = 0; w < kCapWords; w++)
+        caps += (uint32_t)__builtin_popcount(m[w]);
+      if(caps == 0)
+        continue;
+      any = true;
+      if(caps == kCapMicro)
+        refOfRec[r0 + r] = kCapAll;
+      else
+      {
+        refOfRec[r0 + r] = (uint32_t)packed.size();
+        packed.insert(packed.end(), m, m + kCapWords);
+      }
+    }
+  }
+  if(!any)
+    return B200PT_OK;
+  std::vector<uint32_t> recOfSlot(nC), refC(nC, kCapNone), refS(nS, kCapNone);
+  CK(cudaMemcpy(recOfSlot.data(), S.alphaIdx, nC * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  for(uint32_t k = 0; k < nC; k++)
+    if(recOfSlot[k] != 0xFFFFFFFFu)
+      refC[k] = refOfRec[recOfSlot[k]];
+  for(uint32_t r = 0; r < nA; r++)
+    if(shadowOk[r])
+      refS[base + r] = refOfRec[r];
+  DeviceArena     caps;
+  const uint32_t* dRefC = caps.upload(refC.data(), refC.size(), st);
+  const uint32_t* dRefS = caps.upload(refS.data(), refS.size(), st);
+  const uint32_t* dPacked = caps.upload(packed.data(), packed.size(), st);
+  if(!caps.ok())
+    return failed(h, caps, "alpha caps");
+  CK(cudaStreamSynchronize(st));  // (the uploads read the host vectors)
+  h->capMem = std::move(caps);
+  S.bvh.capRef = dRefC;
+  S.bvh.capBits = dPacked;
+  S.bvhA.capRef = dRefS;
+  S.bvhA.capBits = dPacked;
+  return B200PT_OK;
+}
+
+// The caps of a scene that has just been committed (b200pt_set_scene, a scene edit).  The scene is complete and renders exactly the same
+// without them, so a failed bake (an allocation or a copy) does not undo or fail the call that committed it: the walks then run without
+// caps until the next bake, and the failure stays readable in b200pt_last_error.
+void commitAlphaCaps(b200pt* h)
+{
+  if(bakeAlphaCaps(h))
+  {
+    for(BvhView* v : {&h->S.bvh, &h->S.bvhO, &h->S.bvhA})
+      v->capRef = v->capBits = nullptr;
+    h->capMem.release();
+    cudaGetLastError();
+    h->err = "alpha caps not baked (the scene renders without them): " + h->err;
+  }
+}
+
 }  // namespace
 extern "C" {
 
@@ -3450,6 +3574,7 @@ int b200pt_set_scene(b200pt_t* h, const b200pt_scene_desc* s)
     return rc;
   commitScene(h, *s, b);
   setTreeWindow(h);
+  commitAlphaCaps(h);
   return B200PT_OK;
 }
 
@@ -3789,6 +3914,29 @@ int loadGeometry(b200pt* h, CurrentScene& c)
   return B200PT_OK;
 }
 
+// what the alpha record and the shadow cap reference of a triangle read from its material (alphaRecOf, the transmission test of
+// bakeAlphaCaps) is the same for material ma of scene a and material mb of scene b
+bool sameAlphaInputs(const b200pt_scene_desc& a, uint32_t ma, const b200pt_scene_desc& b, uint32_t mb)
+{
+  const b200pt_shade_material &x = a.materials[ma], &y = b.materials[mb];
+  auto bits = [](float f) {
+    uint32_t u;
+    memcpy(&u, &f, 4);
+    return u;
+  };
+  auto slot = [](const b200pt_shade_material& m) { return m.pbrModel == 1 ? m.pbrDiffuseTexture : m.pbrBaseColorTexture; };
+  auto factor = [](const b200pt_shade_material& m) { return m.pbrModel == 1 ? m.pbrDiffuseFactor[3] : m.pbrBaseColorFactor[3]; };
+  if(x.alphaMode != y.alphaMode || bits(x.alphaCutoff) != bits(y.alphaCutoff) || x.pbrModel != y.pbrModel || bits(factor(x)) != bits(factor(y))
+     || bits(x.transmissionFactor) != bits(y.transmissionFactor) || slot(x) != slot(y))
+    return false;
+  const uint16_t s = slot(x);
+  if(s == 0)
+    return true;
+  if(s >= a.numTextureInfos || s >= b.numTextureInfos)
+    return s >= a.numTextureInfos && s >= b.numTextureInfos;
+  return a.textureInfos[s].index == b.textureInfos[s].index && a.textureInfos[s].texCoord == b.textureInfos[s].texCoord;
+}
+
 // Applies an edit whose every argument has been checked: `next` is the current scene `cur` with the edit applied.  newTables:
 // next's materials / texture infos replace the tables; newIds: the render nodes' material ids (`next`'s) are written to the device
 // nodes and the hierarchy's mappings.  The replacements are built before anything is swapped, so a failed allocation leaves the
@@ -3807,6 +3955,11 @@ int applySceneEdit(b200pt* h, const char* who, CurrentScene& cur, const b200pt_s
   if(rebuild)
     if(const int rc = validateMicromaps(h, who, next))
       return rc;
+  // the alpha caps follow the alpha records: baked again after a rebuild, or when an in-place edit changed an alpha input of a visible node
+  bool rebake = rebuild;
+  for(uint32_t n = 0; n < old.numRenderNodes && !rebake; n++)
+    if(next.renderNodeVisible[n] && old.renderPrimitives[next.renderNodes[n].renderPrimID].triangleCount)
+      rebake = !sameAlphaInputs(old, materialOf(old.renderNodes[n]), next, materialOf(next.renderNodes[n]));
   const cudaStream_t st = h->stream;
   DeviceArena        tables;
   const b200pt_shade_material* dMats = h->S.mats;
@@ -3829,7 +3982,7 @@ int applySceneEdit(b200pt* h, const char* who, CurrentScene& cur, const b200pt_s
     if((rc = loadGeometry(h, cur)) || (rc = buildTreeArena(h, next, b)))
       return rc;
   }
-  // nothing below allocates
+  // nothing below allocates but the alpha-cap bake at the end, whose failure only leaves the committed scene without caps (commitAlphaCaps)
   if(newIds && next.numRenderNodes)
   {
     CK(cudaMemcpy2DAsync(reinterpret_cast<char*>(h->dNodesW) + offsetof(b200pt_render_node, materialID), sizeof(b200pt_render_node), newIds, sizeof(int32_t),
@@ -3875,6 +4028,9 @@ int applySceneEdit(b200pt* h, const char* who, CurrentScene& cur, const b200pt_s
   }
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(st));
+  // (a stale map would make the walks skip what they must find; a rebuild's new arena starts without caps)
+  if(rebake)
+    commitAlphaCaps(h);
   return B200PT_OK;
 }
 

@@ -6,6 +6,7 @@
 // bound".  The any-hit loops of the reference (stochastic alpha, coloured transmission) become
 // front-to-back iterations of that query, which makes the result independent of tree layout.
 #pragma once
+#include "alpha_caps.cuh"
 #include "bvh.h"
 #include "omm.cuh"
 #include "vec.cuh"
@@ -39,6 +40,9 @@ struct BvhView
   // opacity micromaps (omm.cuh): one reference word per triangle slot of THIS tree and the packed states; nullptr = the scene has none
   const uint32_t* __restrict__ ommRef = nullptr;
   const uint8_t* __restrict__ ommData = nullptr;
+  // alpha caps (alpha_caps.cuh): one reference word per triangle slot of THIS tree and the bit maps; nullptr = no caps
+  const uint32_t* __restrict__ capRef = nullptr;
+  const uint32_t* __restrict__ capBits = nullptr;
 };
 
 PT_D uint32_t extractByte(uint32_t x, int i) { return (x >> (i * 8)) & 0xffu; }
@@ -202,9 +206,12 @@ struct TravState
   // MODE: the walk's protocol as a compile-time constant where the caller knows it (0 = the runtime flags of init(); 1 = closest-hit
   // walk: not a shadow query, back faces culled, the bound shrinks; 2 = shadow walk: shadow query, no culling) -- the per-triangle
   // flag tests and the shadow / closest branches fold away
-  template <int KC = kCand, bool FORCE_OPAQUE = false, bool OMM = false, int MODE = 0>
+  // CAPS: the scene carries alpha caps (alpha_caps.cuh): a kept candidate whose micro-triangle is a cap lowers the bound of a walk
+  // whose bound shrinks (its own instantiation, so that scenes without non-opaque triangles run the walk without the lookup)
+  template <int KC = kCand, bool FORCE_OPAQUE = false, bool OMM = false, int MODE = 0, bool CAPS = false>
   PT_D bool step(uint2* __restrict__ stack, int postponeShift, Cand* __restrict__ cand, int cs, const uint32_t* __restrict__ ommRef = nullptr,
-                 const uint8_t* __restrict__ ommData = nullptr)
+                 const uint8_t* __restrict__ ommData = nullptr, const uint32_t* __restrict__ capRef = nullptr,
+                 const uint32_t* __restrict__ capBits = nullptr)
   {
     const bool shadow = MODE == 1 ? false : (MODE == 2 ? true : this->shadow);
     const bool cull = MODE == 1 ? true : (MODE == 2 ? false : this->cull);
@@ -419,6 +426,18 @@ struct TravState
                 collectN++;
               if(collectN == KC && shrink)
                 bound = fminf(bound, cand[(KC - 1) * cs].t);
+              // a cap passes its any-hit test whatever it draws: nothing behind it is drawn for, so nothing behind it is needed
+              // (the (t, id) order is kept: the box test's widening still admits triangles at t itself)
+              if(CAPS && shrink)
+              {
+                const uint32_t ref = __ldg(&capRef[slot]);
+                if(ref != kCapNone)
+                {
+                  const bool fl = (flags & TRI_FLIPPED) != 0;
+                  if(capAt(ref, fl ? v : u, fl ? u : v, [&](uint32_t o) { return __ldg(&capBits[o]); }))
+                    bound = fminf(bound, t);
+                }
+              }
             }
           }
         }
