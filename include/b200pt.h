@@ -615,6 +615,13 @@ int b200pt_trace_closest(b200pt_t* h, const float* dev_rays, uint32_t n, float* 
 /* TraceShadow semantics (:139-187): writes rgb transmission (3 floats per ray). */
 int b200pt_trace_shadow(b200pt_t* h, const float* dev_rays, uint32_t n, float* dev_transmission, uint32_t* dev_seeds);
 
+/* Hit-state unit-test hook: n rays traced as b200pt_trace_closest traces them, then the shade kernel's hit fetch,
+ * getHitState, ray-cone texture gradient and evaluateMaterial in the feature variant frames of the current scene run.
+ * in: 16 floats per item (the 8 floats of the ray, isInside, coneWidth, pixelAngle, texGradScale, 4 unused); out: 96 floats
+ * per item (see vk_gltf_renderer_b200/shade_io.py); seeds as for b200pt_trace_closest.  Device pointers.
+ * B200PT_E_INVALID without a scene or buffers. */
+int b200pt_shade_state(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out, uint32_t* dev_seeds);
+
 /* Size in bytes of the traversal structure (nodes, triangles) for the roofline model. */
 int b200pt_bvh_info(b200pt_t* h, uint64_t* node_bytes, uint64_t* tri_bytes, uint32_t* num_nodes, uint32_t* num_tris);
 

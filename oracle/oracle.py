@@ -59,6 +59,7 @@ def lib():
         L.oracle_safe_offset_ray.argtypes = [C.c_void_p] * 3
         L.oracle_sample_texture.argtypes = [C.c_void_p, C.c_int, C.c_float, C.c_float, C.c_float, C.c_void_p]
         L.oracle_texture_lookup.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+        L.oracle_shade_state.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -211,6 +212,14 @@ class Oracle:
         out = np.empty((len(records), 4), np.float32)
         if self.L.oracle_texture_lookup(self.h, _p(records), len(records), _p(out)):
             raise ValueError("oracle_texture_lookup: a record has a texture-info slot outside the scene or a mode other than 0 / 1")
+        return out
+
+    def shade_state(self, records, seeds=None):
+        """closest hit, getHitState, texture gradient and evaluateMaterial on the records of vk_gltf_renderer_b200.shade_io:
+        float32 [n, 96]; seeds (uint32 [n], the any-hit draws) are advanced in place"""
+        records = np.ascontiguousarray(records, np.float32).reshape(-1, 16)
+        out = np.empty((len(records), 96), np.float32)
+        self.L.oracle_shade_state(self.h, _p(records), len(records), _p(out), _p(seeds))
         return out
 
     def hg_sample(self, records):

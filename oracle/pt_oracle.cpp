@@ -2847,4 +2847,106 @@ int oracle_texture_lookup(void* h, const float* in, uint32_t n, float* out)
   }
   return 0;
 }
+
+// hit-state unit hook: per record the closest hit, getHitState, the ray-cone texture gradient and evaluateMaterial, called as
+// the bounce calls them (layout: vk_gltf_renderer_b200/shade_io.py)
+static void putShadeField(float* q, int at, float3 v)
+{
+  q[at] = v.x;
+  q[at + 1] = v.y;
+  q[at + 2] = v.z;
+}
+int oracle_shade_state(void* h, const float* in, uint32_t n, float* out, uint32_t* seeds)
+{
+  Oracle& o = *(Oracle*)h;
+  for(uint32_t i = 0; i < n; i++)
+  {
+    const float* p = in + (size_t)i * 16;
+    float*       q = out + (size_t)i * 96;
+    Ray          r;
+    r.o = f3(p[0], p[1], p[2]);
+    r.tmin = p[3];
+    r.d = f3(p[4], p[5], p[6]);
+    r.tmax = p[7];
+    uint32_t   seed = seeds ? seeds[i] : 0;
+    HitPayload pl;
+    Trace(o, r, pl, seed);
+    if(seeds)
+      seeds[i] = seed;
+    std::fill(q, q + 96, 0.0f);
+    q[0] = pl.hitT;
+    q[1] = (float)pl.rnodeID;
+    q[2] = (float)pl.rprimID;
+    q[3] = (float)pl.primitiveID;
+    if(pl.hitT == INFINITE_F)
+      continue;
+    q[4] = pl.bx;
+    q[5] = pl.by;
+    const b200pt_render_node& rn = o.nodes[pl.rnodeID];
+    const HitState hit = getHitState(o.prims[pl.rprimID], f3(1.0f - pl.bx - pl.by, pl.bx, pl.by), *(const mat4*)rn.worldToObject,
+                                     *(const mat4*)rn.objectToWorld, (uint32_t)pl.primitiveID, r.d);
+    const float    worldFoot = (p[9] + p[10] * pl.hitT) / fmaxf(fabsf(dot(hit.geonrm, -r.d)), 1e-3f);
+    MeshState      mesh;
+    mesh.N = hit.nrm;
+    mesh.T = hit.tangent;
+    mesh.B = hit.bitangent;
+    mesh.Ng = hit.geonrm;
+    mesh.tc[0] = hit.uv[0];
+    mesh.tc[1] = hit.uv[1];
+    mesh.isInside = p[8] != 0.0f;
+    mesh.texGrad = worldFoot * hit.texelDensity * p[11];
+    mesh.baseColorVertexMul = hit.color;
+    const PbrMaterial m = evaluateMaterial(o, o.mats[std::max(0, rn.materialID)], mesh);
+    putShadeField(q, 6, hit.pos);
+    putShadeField(q, 9, hit.nrm);
+    q[12] = hit.color.x;
+    q[13] = hit.color.y;
+    q[14] = hit.color.z;
+    q[15] = hit.color.w;
+    putShadeField(q, 16, hit.geonrm);
+    putShadeField(q, 19, hit.shadowPos);
+    q[22] = hit.uv[0].x;
+    q[23] = hit.uv[0].y;
+    q[24] = hit.uv[1].x;
+    q[25] = hit.uv[1].y;
+    putShadeField(q, 26, hit.tangent);
+    putShadeField(q, 29, hit.bitangent);
+    q[32] = hit.texelDensity;
+    q[33] = mesh.texGrad;
+    putShadeField(q, 34, m.baseColor);
+    q[37] = m.opacity;
+    q[38] = m.roughness.x;
+    q[39] = m.roughness.y;
+    q[40] = m.metallic;
+    putShadeField(q, 41, m.emissive);
+    putShadeField(q, 44, m.N);
+    putShadeField(q, 47, m.T);
+    putShadeField(q, 50, m.B);
+    putShadeField(q, 53, m.Ng);
+    q[56] = m.ior1;
+    q[57] = m.ior2;
+    q[58] = m.specular;
+    putShadeField(q, 59, m.specularColor);
+    q[62] = m.transmission;
+    putShadeField(q, 63, m.attenuationColor);
+    q[66] = m.attenuationDistance;
+    q[67] = m.thickness;
+    q[68] = m.clearcoat;
+    q[69] = m.clearcoatRoughness;
+    putShadeField(q, 70, m.Nc);
+    q[73] = m.iridescence;
+    q[74] = m.iridescenceIor;
+    q[75] = m.iridescenceThickness;
+    putShadeField(q, 76, m.sheenColor);
+    q[79] = m.sheenRoughness;
+    q[80] = m.dispersion;
+    q[81] = m.diffuseTransmissionFactor;
+    putShadeField(q, 82, m.diffuseTransmissionColor);
+    putShadeField(q, 85, m.scatterCoefficient);
+    q[88] = m.scatterAnisotropy;
+    q[89] = m.retroreflection;
+  }
+  o.stats.merge();
+  return 0;
+}
 }

@@ -17,7 +17,7 @@ EXPORTS = [
     "b200pt_set_environment", "b200pt_resize", "b200pt_resize_interleaved", "b200pt_read_accum_async", "b200pt_wait_read", "b200pt_set_frames_in_flight", "b200pt_render_frame", "b200pt_synchronize",
     "b200pt_get_accum_device", "b200pt_read_accum", "b200pt_set_accum_device", "b200pt_stream",
     "b200pt_get_stats", "b200pt_reset_stats", "b200pt_set_profiling", "b200pt_trace_closest",
-    "b200pt_trace_shadow", "b200pt_bvh_info", "b200pt_bsdf_eval", "b200pt_bsdf_sample", "b200pt_texture_lookup",
+    "b200pt_trace_shadow", "b200pt_bvh_info", "b200pt_bsdf_eval", "b200pt_bsdf_sample", "b200pt_texture_lookup", "b200pt_shade_state",
     "b200pt_read_selection", "b200pt_get_selection_device", "b200pt_set_frame_batch", "b200pt_flush", "b200pt_update_transforms", "b200pt_set_bvh_builder", "b200pt_bvh_build_ms",
     "b200pt_set_opacity_micromaps", "b200pt_set_animation", "b200pt_animate", "b200pt_set_node_hierarchy", "b200pt_update_node_matrices", "b200pt_tonemap", "b200pt_tonemap_image", "b200pt_get_tonemapped_device", "b200pt_set_guide_outputs", "b200pt_read_guide", "b200pt_get_guide_device",
     "b200pt_set_dlss_guides", "b200pt_read_dlss_guides", "b200pt_get_dlss_guides_device",
@@ -77,6 +77,7 @@ def lib(count_traversal=False):
     L.b200pt_bsdf_eval.argtypes = [vp, vp, u32, vp]
     L.b200pt_bsdf_sample.argtypes = [vp, vp, u32, vp]
     L.b200pt_texture_lookup.argtypes = [vp, vp, u32, vp]
+    L.b200pt_shade_state.argtypes = [vp, vp, u32, vp, vp]
     L.b200pt_read_selection.argtypes = [vp, vp, vp, C.c_size_t]
     L.b200pt_set_frame_batch.argtypes = [vp, i32]
     L.b200pt_flush.argtypes = [vp]

@@ -756,10 +756,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     }
 
     // ---- hit-attribute fetch ----
-    meta = S.triMeta[slot];
-    nodeP = &S.nodes[meta.x & 0x0fffffffu];
-    const b200pt_render_node& node = *nodeP;
-    const ShadeRec            srec = loadShadeRec(S.shadeRecs + __ldg(&S.shadeIdx[slot]));
+    hit = fetchHitState(S, slot, hr.y, hr.z, dir, meta, nodeP);
 #ifdef B200PT_DEBUG
     // reference analogue: doDebug at pushConst.mouseCoord (gltf_pathtrace.slang:553-557)
     dbgPixel = ((float)(pixelOf(F, i) % (uint32_t)F.width) == F.pc.mouseCoord[0] && (float)pixelRow(F, pixelOf(F, i)) == F.pc.mouseCoord[1]);
@@ -767,14 +764,12 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
       printf("DBG hit t=%.9g rnode=%d prim=%d bary=%.9g %.9g org=%.9g %.9g %.9g dir=%.9g %.9g %.9g seed=%u depth=%d\n", hitT, (int)(meta.x & 0x0fffffffu), (int)meta.y, hr.y, hr.z,
              org.x, org.y, org.z, dir.x, dir.y, dir.z, seed, (int)depth);
 #endif
-    const float3              bary = f3(1.0f - hr.y - hr.z, hr.y, hr.z);
-    hit = getHitState(srec, bary, node.worldToObject, node.objectToWorld, dir);
     statAdd(&stats->shadedHits, 1ull);
     return true;
   };
   // ---- section 2: material evaluation (three trilinear texture lookups), emission, unlit ----
   auto shadeMaterial = [&]() -> bool {
-    worldFoot = (coneWidth + F.pc.pixelAngle * hitT) / fmaxf(fabsf(dot(hit.geonrm, -dir)), 1e-3f);
+    worldFoot = rayConeWorldFootprint(coneWidth, F.pc.pixelAngle, hitT, hit.geonrm, dir);
     int unlit = 0;
     if(onPlane)
     {
@@ -791,7 +786,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     {
       const b200pt_render_node&    node = *nodeP;
       const int                    materialIndex = max(0, node.materialID);
-      const float                  texGrad = worldFoot * hit.texelDensity * F.pc.texGradScale;
+      const float                  texGrad = footprintTexGrad(worldFoot, hit.texelDensity, F.pc.texGradScale);
       const b200pt_shade_material& gmat = S.mats[materialIndex];
       pbrMat = evaluateMaterial<FEAT>(S, gmat, hit, (flags & PF_INSIDE) != 0, texGrad);
       unlit = gmat.unlit;
@@ -1652,13 +1647,14 @@ __global__ void __launch_bounds__(256) k_cap_bake(const AlphaRec* __restrict__ r
 
 // ---- ray-level API (parity tests / traversal micro-benchmark): the rays run through the PRODUCTION kernels
 // (k_trace / k_shadow -> k_alpha -> continuation round -> k_alpha) on a scratch path pool -------------------------
-__global__ void __launch_bounds__(256) k_rays_load(PathState P, const float4* __restrict__ rays, uint32_t n, const uint32_t* __restrict__ seeds, uint32_t* q, uint32_t* cnt,
-                                                   int shadow)
+// rays: recordFloat4s float4 per record, the first two the ray
+__global__ void __launch_bounds__(256) k_rays_load(PathState P, const float4* __restrict__ rays, uint32_t recordFloat4s, uint32_t n, const uint32_t* __restrict__ seeds,
+                                                   uint32_t* q, uint32_t* cnt, int shadow)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
   for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride)
   {
-    const float4 o = rays[i * 2], d = rays[i * 2 + 1];
+    const float4 o = rays[i * recordFloat4s], d = rays[i * recordFloat4s + 1];
     if(!shadow)
     {
       P.rayO[i] = o;  // .w = tmin (TRACE_TMIN)
@@ -1716,6 +1712,98 @@ __global__ void __launch_bounds__(256) k_rays_store(PathState P, DevScene S, uin
     o[4] = u;
     o[5] = v;
   }
+}
+
+// hit-state unit-test hook: the closest hit of a traced ray through k_shade's hit fetch, footprint and material evaluation
+// (layout in vk_gltf_renderer_b200/shade_io.py)
+PT_D void putShadeField(float* q, int at, float3 v)
+{
+  q[at] = v.x;
+  q[at + 1] = v.y;
+  q[at + 2] = v.z;
+}
+template <uint32_t FEAT>
+__global__ void __launch_bounds__(128) k_shade_state(PathState P, DevScene S, const float* __restrict__ in, uint32_t n, float* __restrict__ out, uint32_t* seeds)
+{
+  stageSrgbLut(S.lutSrgb);
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if(i >= n)
+    return;
+  if(seeds)
+    seeds[i] = __float_as_uint(P.misc[i].w);
+  const float*   p = in + (size_t)i * 16;
+  float*         q = out + (size_t)i * 96;
+  const float4   hr = P.hit[i];
+  const uint32_t slot = __float_as_uint(hr.w);
+  for(int k = 0; k < 96; k++)
+    q[k] = 0.0f;
+  if(slot == 0xFFFFFFFFu)
+  {
+    q[0] = kInfinite;
+    q[1] = q[2] = q[3] = -1.0f;
+    return;
+  }
+  const float3              dir = f3(p[4], p[5], p[6]);
+  uint2                     meta;
+  const b200pt_render_node* nodeP;
+  const HitState            hit = fetchHitState(S, slot, hr.y, hr.z, dir, meta, nodeP);
+  const float               worldFoot = rayConeWorldFootprint(p[9], p[10], hr.x, hit.geonrm, dir);
+  const float               texGrad = footprintTexGrad(worldFoot, hit.texelDensity, p[11]);
+  const PbrMaterial         m = evaluateMaterial<FEAT>(S, S.mats[max(0, nodeP->materialID)], hit, p[8] != 0.0f, texGrad);
+  q[0] = hr.x;
+  q[1] = (float)(meta.x & 0x0fffffffu);
+  q[2] = (float)nodeP->renderPrimID;
+  q[3] = (float)meta.y;
+  q[4] = hr.y;
+  q[5] = hr.z;
+  putShadeField(q, 6, hit.pos);
+  putShadeField(q, 9, hit.nrm);
+  q[12] = hit.color.x;
+  q[13] = hit.color.y;
+  q[14] = hit.color.z;
+  q[15] = hit.color.w;
+  putShadeField(q, 16, hit.geonrm);
+  putShadeField(q, 19, hit.shadowPos);
+  q[22] = hit.uv0.x;
+  q[23] = hit.uv0.y;
+  q[24] = hit.uv1.x;
+  q[25] = hit.uv1.y;
+  putShadeField(q, 26, hit.tangent);
+  putShadeField(q, 29, hit.bitangent);
+  q[32] = hit.texelDensity;
+  q[33] = texGrad;
+  putShadeField(q, 34, m.baseColor);
+  q[37] = m.opacity;
+  q[38] = m.roughness.x;
+  q[39] = m.roughness.y;
+  q[40] = m.metallic;
+  putShadeField(q, 41, m.emissive);
+  putShadeField(q, 44, m.N);
+  putShadeField(q, 47, m.T);
+  putShadeField(q, 50, m.B);
+  putShadeField(q, 53, m.Ng);
+  q[56] = m.ior1;
+  q[57] = m.ior2;
+  q[58] = m.specular;
+  putShadeField(q, 59, m.specularColor);
+  q[62] = m.transmission;
+  putShadeField(q, 63, m.attenuationColor);
+  q[66] = m.attenuationDistance;
+  q[67] = m.thickness;
+  q[68] = m.clearcoat;
+  q[69] = m.clearcoatRoughness;
+  putShadeField(q, 70, m.Nc);
+  q[73] = m.iridescence;
+  q[74] = m.iridescenceIor;
+  q[75] = m.iridescenceThickness;
+  putShadeField(q, 76, m.sheenColor);
+  q[79] = m.sheenRoughness;
+  q[80] = m.dispersion;
+  q[81] = m.diffuseTransmissionFactor;
+  putShadeField(q, 82, m.diffuseTransmissionColor);
+  putShadeField(q, 85, m.scatterCoefficient);
+  q[88] = m.scatterAnisotropy;
+  q[89] = m.retroreflection;
 }
 
 // packing of the BSDF test records: vk_gltf_renderer_b200/bsdf_io.py
@@ -2863,6 +2951,10 @@ uint32_t featureMaskOf(const b200pt_scene_desc& s)
   }
   return feat;
 }
+
+// the feature variant of the shade kernel a frame runs: k_shade<0> when no material uses an extension feature, k_shade<FEAT_LEAN>
+// when clearcoat is the only one, k_shade<FEAT_ALL> otherwise
+static uint32_t shadeFeatures(const b200pt* h) { return h->featureMask == 0 ? 0u : h->leanShade ? (uint32_t)FEAT_LEAN : (uint32_t)FEAT_ALL; }
 
 // the AoS tables (same bytes as the reference SSBOs) and the vertex data: separate attribute arrays per primitive, as
 // SceneVk::createVertexBuffers
@@ -4934,7 +5026,8 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   if(pc->maxDepth > 0)
   {
     const int gS = gridFor(h, kShadeCtasPerSM);  // persistent shade kernel
-    const auto shade = h->featureMask == 0 ? k_shade<0u> : h->leanShade ? k_shade<FEAT_LEAN> : k_shade<FEAT_ALL>;
+    const uint32_t feat = shadeFeatures(h);
+    const auto     shade = feat == 0u ? k_shade<0u> : feat == FEAT_LEAN ? k_shade<FEAT_LEAN> : k_shade<FEAT_ALL>;
     const bool        sortShade = h->sortShade && h->S.numMaterials + 1 <= kSortMaxBuckets;
     int               cur = 0;  // dQ[cur] = trace queue, dQ[2] = post queue, dQ[1-cur] = next queue
     // (a shadowed shadow-catcher hit continues without consuming depth: such a frame can need more iterations than maxDepth)
@@ -5100,6 +5193,22 @@ static int ensureRayPool(b200pt_t* h, uint32_t n)
   return B200PT_OK;
 }
 
+// the walk of n rays (records of recordFloats floats, the ray first) into the ray pool; the caller reads the pool out
+static int walkRays(b200pt_t* h, const float* dev_rays, uint32_t recordFloats, uint32_t n, uint32_t* dev_seeds, int shadow, const Launcher& ctx)
+{
+  const int rc = ensureRayPool(h, n);
+  if(rc)
+    return rc;
+  const Counters C{h->rayCounters, 1};
+  CK(cudaMemsetAsync(h->rayCounters, 0, sizeof(uint32_t) * kCounterArrays, h->stream));
+  ctx(kStageOther, [&](cudaStream_t st) {
+    k_rays_load<<<gridFor(h, 8), 256, 0, st>>>(h->rayP, reinterpret_cast<const float4*>(dev_rays), recordFloats / 4, n, dev_seeds, h->rayQ[0],
+                                               C.queue(shadow, 0), shadow);
+  });
+  launchWalk(ctx, shadow, h->rayP, h->rayQ[0], h->rayQ[1], h->rayQ[2], C, 0, shadow ? 0 : TRACE_TMIN);
+  return B200PT_OK;
+}
+
 static int traceRays(b200pt_t* h, const float* dev_rays, uint32_t n, float* dev_out, uint32_t* dev_seeds, int shadow)
 {
   if(!h || !h->haveScene || !dev_rays || !dev_out)
@@ -5107,16 +5216,9 @@ static int traceRays(b200pt_t* h, const float* dev_rays, uint32_t n, float* dev_
   CK(cudaSetDevice(h->device));
   if(n == 0)
     return B200PT_OK;
-  const int rc = ensureRayPool(h, n);
-  if(rc)
-    return rc;
-  const Counters C{h->rayCounters, 1};
-  CK(cudaMemsetAsync(h->rayCounters, 0, sizeof(uint32_t) * kCounterArrays, h->stream));
   const Launcher ctx{h, h->stream, -1, 0, -1, false, n};
-  ctx(kStageOther, [&](cudaStream_t st) {
-    k_rays_load<<<gridFor(h, 8), 256, 0, st>>>(h->rayP, reinterpret_cast<const float4*>(dev_rays), n, dev_seeds, h->rayQ[0], C.queue(shadow, 0), shadow);
-  });
-  launchWalk(ctx, shadow, h->rayP, h->rayQ[0], h->rayQ[1], h->rayQ[2], C, 0, shadow ? 0 : TRACE_TMIN);
+  if(const int rc = walkRays(h, dev_rays, 8, n, dev_seeds, shadow, ctx))
+    return rc;
   ctx(kStageOther, [&](cudaStream_t st) { k_rays_store<<<gridFor(h, 8), 256, 0, st>>>(h->rayP, h->S, n, dev_out, dev_seeds, shadow); });
   CK(cudaGetLastError());
   return B200PT_OK;
@@ -5130,6 +5232,28 @@ int b200pt_trace_closest(b200pt_t* h, const float* dev_rays, uint32_t n, float* 
 int b200pt_trace_shadow(b200pt_t* h, const float* dev_rays, uint32_t n, float* dev_transmission, uint32_t* dev_seeds)
 {
   return traceRays(h, dev_rays, n, dev_transmission, dev_seeds, 1);
+}
+
+int b200pt_shade_state(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out, uint32_t* dev_seeds)
+{
+  if(!h)
+    return B200PT_E_INVALID;
+  if(!dev_in || !dev_out || !h->haveScene)
+  {
+    h->err = "b200pt_shade_state: needs a scene and device buffers";
+    return B200PT_E_INVALID;
+  }
+  CK(cudaSetDevice(h->device));
+  if(n == 0)
+    return B200PT_OK;
+  const Launcher ctx{h, h->stream, -1, 0, -1, false, n};
+  if(const int rc = walkRays(h, dev_in, 16, n, dev_seeds, 0, ctx))
+    return rc;
+  const uint32_t feat = shadeFeatures(h);
+  const auto     shade = feat == 0u ? k_shade_state<0u> : feat == FEAT_LEAN ? k_shade_state<FEAT_LEAN> : k_shade_state<FEAT_ALL>;
+  ctx(kStageOther, [&](cudaStream_t st) { shade<<<(n + 127) / 128, 128, 2048, st>>>(h->rayP, h->S, dev_in, n, dev_out, dev_seeds); });
+  CK(cudaGetLastError());
+  return B200PT_OK;
 }
 
 int b200pt_bsdf_eval(b200pt_t* h, const float* dev_in, uint32_t n, float* dev_out)

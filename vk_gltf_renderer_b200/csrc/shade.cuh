@@ -142,6 +142,26 @@ PT_D HitState getHitState(const ShadeRec& R, float3 bary, const float* W2O, cons
   return hit;
 }
 
+// the closest hit's attributes: triangle slot -> render node (triMeta) and gathered attribute record (shadeIdx), barycentrics
+// (1 - u - v, u, v)
+PT_D HitState fetchHitState(const DevScene& S, uint32_t slot, float u, float v, float3 dir, uint2& meta, const b200pt_render_node*& nodeP)
+{
+  meta = S.triMeta[slot];
+  nodeP = &S.nodes[meta.x & 0x0fffffffu];
+  const b200pt_render_node& node = *nodeP;
+  const ShadeRec            srec = loadShadeRec(S.shadeRecs + __ldg(&S.shadeIdx[slot]));
+  const float3              bary = f3(1.0f - u - v, u, v);
+  return getHitState(srec, bary, node.worldToObject, node.objectToWorld, dir);
+}
+
+// rayConeWorldFootprint (nvshaders, gltf_pathtrace.slang:164): the cone's width at the hit over the slant of the surface
+PT_D float rayConeWorldFootprint(float coneWidth, float coneSpread, float hitT, float3 geonrm, float3 dir)
+{
+  return (coneWidth + coneSpread * hitT) / fmaxf(fabsf(dot(geonrm, -dir)), 1e-3f);
+}
+// the SampleGrad gradient of the hit's textures (gltf_pathtrace.slang:196)
+PT_D float footprintTexGrad(float worldFoot, float texelDensity, float texGradScale) { return worldFoot * texelDensity * texGradScale; }
+
 // ---- textures -----------------------------------------------------------------------------------
 // 8-bit sRGB EOTF decode table (same fp32 values as the oracle's), staged in shared memory by every kernel
 // that can touch a texture (divergent indices: constant memory would serialise them)

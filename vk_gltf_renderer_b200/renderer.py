@@ -451,6 +451,12 @@ class PathTracer:
         """n texture lookups (records of tex_io, device pointers) against the attached scene: rgba, 4 floats each"""
         self._ck(self._L.b200pt_texture_lookup(self._h, C.c_void_p(in_ptr), n, C.c_void_p(out_ptr)), "b200pt_texture_lookup")
 
+    def shade_state(self, in_ptr, n, out_ptr, seeds_ptr=None):
+        """n rays (records of shade_io, device pointers) through the closest-hit walk, the hit fetch and evaluateMaterial of the
+        attached scene's shade variant: 96 floats each"""
+        self._ck(self._L.b200pt_shade_state(self._h, C.c_void_p(in_ptr), n, C.c_void_p(out_ptr), C.c_void_p(seeds_ptr) if seeds_ptr else None),
+                 "b200pt_shade_state")
+
 
 def render_headless(resources, frames, *, pt=None, device=0, **pt_params):
     """The reference's headless loop (src/main.cpp:133-136 + nvapp frame loop, SURVEY.md §3.1):
