@@ -21,6 +21,15 @@ class B200PTError(RuntimeError):
     pass
 
 
+# the bytes each scene edit hands the library, by the PathTracer method that sends them: update_scene_changes sends an edit only
+# when they differ from what the handle holds
+_EDIT_BYTES = {
+    "update_materials": lambda s: (b"".join(map(bytes, s.materials)), b"".join(map(bytes, s.texture_infos))),
+    "update_lights": lambda s: b"".join(map(bytes, s.lights)),
+    "set_node_visibility": lambda s: bytes(1 if rn.get("visible", True) else 0 for rn in s.render_nodes),
+}
+
+
 @dataclass
 class Settings:
     """Resources::settings (reference src/resources.hpp:82-133) — fields the path tracer reads."""
@@ -84,6 +93,7 @@ class PathTracer:
         self.m_prevMVP = None          # GltfRenderer::m_prevMVP: the previous frame's viewProjMatrix (src/renderer.cpp:682, 703)
         self.ptPerformanceTarget = 1  # 0 interactive (60 FPS), 1 balanced (30), 2 quality (15), 3 max quality (10)
         self.last_frame_gpu_ms = None  # GPU time of the previous frame's path-trace section (the reference reads its profiler)
+        self._held = {}                # what the handle holds, as _EDIT_BYTES sees it
 
     # -- error plumbing (reference: NVVK_CHECK aborts; here: exceptions carrying b200pt_last_error) --
     def _ck(self, rc, what):
@@ -129,6 +139,7 @@ class PathTracer:
         mm, nmm, po, npo, keep = resources.scene.omm_desc()
         self._ck(self._L.b200pt_set_opacity_micromaps(self._h, mm, nmm, po, npo), "b200pt_set_opacity_micromaps")
         self._ck(self._L.b200pt_set_scene(self._h, C.byref(d)), "b200pt_set_scene")
+        self._held = {name: state(resources.scene) for name, state in _EDIT_BYTES.items()}
 
     def set_bvh_builder(self, kind):
         """0: host SAH builder, 1: device LBVH builder (takes effect at the next onSceneInvalidated)"""
@@ -159,6 +170,7 @@ class PathTracer:
         mats = (abi.ShadeMaterial * max(len(scn.materials), 1))(*scn.materials)
         tis = (abi.TextureInfo * max(len(scn.texture_infos), 1))(*scn.texture_infos)
         self._ck(self._L.b200pt_update_materials(self._h, mats, len(scn.materials), tis, len(scn.texture_infos)), "b200pt_update_materials")
+        self._held["update_materials"] = _EDIT_BYTES["update_materials"](scn)
 
     def update_node_materials(self, resources):
         """the render nodes' materialIDs of resources.scene changed (a material variant switch): b200pt_update_node_materials"""
@@ -171,12 +183,22 @@ class PathTracer:
         lights = resources.scene.lights
         arr = (abi.Light * max(len(lights), 1))(*lights)
         self._ck(self._L.b200pt_update_lights(self._h, arr, len(lights)), "b200pt_update_lights")
+        self._held["update_lights"] = _EDIT_BYTES["update_lights"](resources.scene)
 
     def set_node_visibility(self, resources):
         """the render nodes' visibility of resources.scene changed: b200pt_set_node_visibility"""
         vis = np.ascontiguousarray([1 if rn.get("visible", True) else 0 for rn in resources.scene.render_nodes] or [0], np.uint8)
         self._ck(self._L.b200pt_set_node_visibility(self._h, vis.ctypes.data_as(C.POINTER(C.c_uint8)), len(resources.scene.render_nodes)),
                  "b200pt_set_node_visibility")
+        self._held["set_node_visibility"] = _EDIT_BYTES["set_node_visibility"](resources.scene)
+
+    def update_scene_changes(self, resources):
+        """GltfRenderer::updateSceneChanges for the changes animation.apply_pointers makes to resources.scene: update_materials,
+        update_lights and set_node_visibility, each sent only when its bytes differ from what the handle holds.  A visibility change
+        rebuilds the trees (DESIGN.md §2), so a channel holding its value must not send it again every frame."""
+        for name, state in _EDIT_BYTES.items():
+            if self._held.get(name) != state(resources.scene):
+                getattr(self, name)(resources)
 
     def set_animation(self, morph_tasks=(), skin_tasks=()):
         """SceneAnimationVk::createAnimationResources analogue (b200pt_set_animation): uploads the static inputs of the morph /

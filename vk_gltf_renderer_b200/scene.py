@@ -68,6 +68,10 @@ class Scene:
         # KHR_node_visibility: every glTF node's own flag (a loaded scene); a render node is visible when its node and every
         # ancestor are (Scene::traverseSceneWithVisibility)
         self.node_visible = None
+        # a loaded scene's glTF document, and per light the glTF light index and the world matrix of its node: what
+        # animation.apply_pointers converts again when KHR_animation_pointer channels change materials, lights or nodes
+        self.gltf = None
+        self.light_sources = []
         self._keep = []
 
     # -- bounds (reference: Scene::getSceneBounds, gltf_scene.cpp:2303-2336, from transformed vertices)
@@ -450,6 +454,33 @@ def _tex_transform(tinfo):
     return (sx * c, -sy * s, sx * s, sy * c, ox, oy)
 
 
+def make_light(gll, world):
+    """glTF KHR_lights_punctual light (JSON dict) placed by its node's world matrix (math 4x4) -> GltfLight
+    (gltf_scene_vk.cpp:1354-1394)"""
+    L = abi.Light()
+    L.position[:] = world[:3, 3].tolist()
+    L.direction[:] = (-world[:3, 2]).tolist()
+    spot = gll.get("spot", {})
+    L.innerAngle = spot.get("innerConeAngle", 0.0)
+    L.outerAngle = spot.get("outerConeAngle", math.pi / 4)
+    L.color[:] = gll.get("color", [1, 1, 1])
+    L.intensity = gll.get("intensity", 1.0)
+    L.type = {"point": 3, "spot": 2}.get(gll.get("type"), 1)
+    ex = gll.get("extras")
+    L.radius = float(ex.get("radius", 0.0)) if isinstance(ex, dict) else 0.0
+    if L.type == 1:
+        L.angularSizeOrInvRange = 2.0 * math.atan(L.radius / 149597870.0)
+    else:
+        rng = gll.get("range", 0.0)
+        L.angularSizeOrInvRange = 1.0 / rng if rng > 0 else 0.0
+    return L
+
+
+def node_visible(node):
+    """KHR_node_visibility flag of one glTF node (JSON dict), its own, not inherited"""
+    return bool(node.get("extensions", {}).get("KHR_node_visibility", {}).get("visible", True))
+
+
 def populate_shade_material(sm, add_texture_info):
     """tinygltf::Material (here: the glTF JSON dict) -> GltfShadeMaterial, field by field like
     MaterialCache::populateShaderMaterial (src/gltf_material_cache.cpp:63-233).  `add_texture_info(index, texCoord,
@@ -807,14 +838,20 @@ def load_gltf(path):
         if "inverseBindMatrices" in sk:
             ibm = g.accessor(sk["inverseBindMatrices"]).astype(np.float64).reshape(-1, 4, 4).transpose(0, 2, 1)   # glm column-major -> (row, col)
         skins.append(dict(joints=list(sk.get("joints", [])), ibm=ibm))
-    # animations as AnimationSystem::parseAnimations caches them: per sampler the key times, the decoded outputs and the interpolation
+    # animations as AnimationSystem::parseAnimations caches them: per sampler the key times, the decoded outputs with their accessor
+    # type and the interpolation; per channel its target, and for a "pointer" channel the KHR_animation_pointer string (empty
+    # without the extension: gltf_scene_animation.cpp:182-188)
     animations = []
     for an in j.get("animations", []):
         samplers = []
         for sm in an.get("samplers", []):
             samplers.append(dict(inputs=g.accessor(sm["input"]).astype(np.float32).reshape(-1), outputs=g.accessor(sm["output"]).astype(np.float32),
-                                 interpolation=sm.get("interpolation", "LINEAR")))
-        channels = [dict(node=ch.get("target", {}).get("node", -1), path=ch.get("target", {}).get("path", ""), sampler=ch["sampler"]) for ch in an.get("channels", [])]
+                                 type=j["accessors"][sm["output"]]["type"], interpolation=sm.get("interpolation", "LINEAR")))
+        channels = []
+        for ch in an.get("channels", []):
+            tgt = ch.get("target", {})
+            pointer = tgt.get("extensions", {}).get("KHR_animation_pointer", {}).get("pointer", "") if tgt.get("path") == "pointer" else ""
+            channels.append(dict(node=tgt.get("node", -1), path=tgt.get("path", ""), sampler=ch["sampler"], pointer=pointer))
         animations.append(dict(name=an.get("name", ""), samplers=samplers, channels=channels))
     scn.graph = dict(parents=parents, locals=np.asarray([_node_matrix(n) for n in nodes], np.float64).reshape(-1, 4, 4), render_nodes=[], skins=skins,
                      mesh_weights={m: np.asarray(mesh.get("weights", []), np.float32) for m, mesh in enumerate(j.get("meshes", []))},
@@ -828,24 +865,8 @@ def load_gltf(path):
             cam_found.append((nid, world))
         li = node.get("extensions", {}).get("KHR_lights_punctual", {}).get("light", -1)
         if 0 <= li < len(gl_lights):
-            gll = gl_lights[li]
-            L = abi.Light()
-            L.position[:] = world[:3, 3].tolist()
-            L.direction[:] = (-world[:3, 2]).tolist()
-            spot = gll.get("spot", {})
-            L.innerAngle = spot.get("innerConeAngle", 0.0)
-            L.outerAngle = spot.get("outerConeAngle", math.pi / 4)
-            L.color[:] = gll.get("color", [1, 1, 1])
-            L.intensity = gll.get("intensity", 1.0)
-            L.type = {"point": 3, "spot": 2}.get(gll.get("type"), 1)
-            ex = gll.get("extras")
-            L.radius = float(ex.get("radius", 0.0)) if isinstance(ex, dict) else 0.0
-            if L.type == 1:
-                L.angularSizeOrInvRange = 2.0 * math.atan(L.radius / 149597870.0)
-            else:
-                rng = gll.get("range", 0.0)
-                L.angularSizeOrInvRange = 1.0 / rng if rng > 0 else 0.0
-            scn.lights.append(L)
+            scn.lights.append(make_light(gl_lights[li], world))
+            scn.light_sources.append((li, world))
         if node.get("mesh", -1) > -1:
             inst = node.get("extensions", {}).get("EXT_mesh_gpu_instancing")
             locals_ = [np.eye(4)]
@@ -873,8 +894,9 @@ def load_gltf(path):
     for root in j.get("scenes", [{"nodes": list(range(len(nodes)))}])[scene_id]["nodes"]:
         visit(root, np.eye(4))
     scn.variants = [v.get("name", "") for v in j.get("extensions", {}).get("KHR_materials_variants", {}).get("variants", [])]
-    scn.node_visible = [bool(n.get("extensions", {}).get("KHR_node_visibility", {}).get("visible", True)) for n in nodes]
+    scn.node_visible = [node_visible(n) for n in nodes]
     scn._apply_visibility()
+    scn.gltf = j
 
     # ---- camera (Scene::handleCameraTraversal) ----
     if cam_found:
