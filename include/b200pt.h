@@ -588,6 +588,29 @@ int b200pt_set_frames_in_flight(b200pt_t* h, int n);
 int b200pt_set_frame_batch(b200pt_t* h, int n);
 int b200pt_flush(b200pt_t* h);
 
+/* Views: n (1..64, default 1) camera poses of one static scene rendered as ONE wavefront of n x pixels paths, each view into its
+ * own images -- stereo pairs, the faces of a probe, turntable rings, dataset poses -- so that small views fill the GPU like one
+ * large frame.  View 0 is the handle's accumulation / selection / depth image (b200pt_read_accum, b200pt_read_selection, ...);
+ * views 1..n-1 get tile-sized RGBA32F, object-id and NDC-depth images of their own.  Like b200pt_set_frame_batch it rebuilds the
+ * path pools (n x pixels slots per lane) and clears every image; B200PT_E_NOMEM if they do not fit (the view count is then
+ * unchanged and, as after a failed b200pt_resize, the next resize rebuilds the pools).  More than one view and frame batching
+ * exclude each other: either call returns B200PT_E_UNSUPPORTED while the other is above 1.
+ *
+ * b200pt_render_views renders one frame of every view; n must equal the view count.  fis[v] is what b200pt_render_frame would
+ * take for view v, and the views may differ ONLY in viewMatrix, viewInv, viewProjMatrix and prevMVP (any other byte that differs:
+ * B200PT_E_INVALID); the push constants are shared.  After any sequence of calls, view v's image, object ids and depth are
+ * bit-identical to what b200pt_render_frame(&fis[v], pc) produces over the same push-constant sequence, and the stats counters are
+ * the sums of those renders.  With more than one view, push constants carrying B200PT_PT_USE_DLSS or B200PT_PT_USE_OPTIX_DENOISER
+ * are refused (B200PT_E_UNSUPPORTED): those guide images belong to one displayed frame.  The call never joins a frame batch;
+ * b200pt_render_frame stays valid and renders view 0.
+ *
+ * b200pt_read_views copies one view's images (tile_rows x width pixels each; any pointer may be NULL); b200pt_get_views_device
+ * returns their device pointers (b200pt_tonemap_image tonemaps them). */
+int b200pt_set_views(b200pt_t* h, int n);
+int b200pt_render_views(b200pt_t* h, const b200pt_frame_info* fis, uint32_t n, const b200pt_push_constant* pc);
+int b200pt_read_views(b200pt_t* h, uint32_t view, float* host_rgba32f, uint32_t* host_object_ids, float* host_ndc_depth, size_t num_pixels);
+int b200pt_get_views_device(b200pt_t* h, uint32_t view, float** dev_rgba32f, uint32_t** dev_object_ids, float** dev_ndc_depth);
+
 /* Let the caller own the accumulation storage (e.g. a torch tensor that NCCL all-gathers):
  * dev_rgba32f must hold tile_rows*width*4 floats on the handle's device. NULL restores the
  * internal buffer. */

@@ -22,6 +22,7 @@ EXPORTS = [
     "b200pt_set_opacity_micromaps", "b200pt_set_animation", "b200pt_animate", "b200pt_set_node_hierarchy", "b200pt_update_node_matrices", "b200pt_tonemap", "b200pt_tonemap_image", "b200pt_get_tonemapped_device", "b200pt_set_guide_outputs", "b200pt_read_guide", "b200pt_get_guide_device",
     "b200pt_set_dlss_guides", "b200pt_read_dlss_guides", "b200pt_get_dlss_guides_device",
     "b200pt_update_materials", "b200pt_update_node_materials", "b200pt_update_lights", "b200pt_set_node_visibility",
+    "b200pt_set_views", "b200pt_render_views", "b200pt_read_views", "b200pt_get_views_device",
 ]
 
 
@@ -102,6 +103,10 @@ def lib(count_traversal=False):
     L.b200pt_read_dlss_guides.argtypes = [vp, C.POINTER(abi.DlssGuides)]
     L.b200pt_get_dlss_guides_device.argtypes = [vp, C.POINTER(abi.DlssGuides)]
     L.b200pt_get_selection_device.argtypes = [vp, C.POINTER(vp), C.POINTER(vp)]
+    L.b200pt_set_views.argtypes = [vp, i32]
+    L.b200pt_render_views.argtypes = [vp, C.POINTER(abi.FrameInfo), u32, C.POINTER(abi.PushConstant)]
+    L.b200pt_read_views.argtypes = [vp, u32, vp, vp, vp, C.c_size_t]
+    L.b200pt_get_views_device.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     for name in EXPORTS:
         getattr(L, name)  # raises AttributeError if a declared symbol is not exported
     _libs[path] = L

@@ -189,6 +189,11 @@ PT_USE_DLSS = 1 << 0
 PT_USE_OPTIX_DENOISER = 1 << 1
 PT_FIRST_FRAME = 1 << 2
 
+# b200pt_set_views / b200pt_render_views: the most views one handle renders at once, and the FrameInfo fields in which the views
+# of one call may differ (every other byte must be equal)
+MAX_VIEWS = 64
+VIEW_POSE_FIELDS = ("viewMatrix", "viewInv", "viewProjMatrix", "prevMVP")
+
 
 def fptr(a):
     """numpy float32 array -> float* (None -> NULL)."""

@@ -6,6 +6,7 @@ Mirrors what GltfRenderer::onRender writes into SceneFrameInfo every frame
 its matrices are glm::lookAt and glm::perspectiveRH_ZO with the Vulkan Y flip ([1][1] *= -1).
 All arithmetic is done in float64 and rounded once to float32.
 """
+import ctypes as C
 import math
 
 import numpy as np
@@ -99,6 +100,22 @@ def make_frame_info(cam, width, height, *, use_hdr=True, env_rotation=0.0, env_i
     fi.infinitePlaneRoughness = plane_roughness
     fi.shadowCatcherDarkenAmount = max(catcher_darkness, 0.0)   # src/renderer.cpp:700
     return fi
+
+
+def view_frame_infos(base, views):
+    """The frame infos of b200pt_render_views: one copy of `base` per view, with that view's pose.  `views` are world-to-camera
+    matrices (4x4, as look_at returns them); the projection is base's (inverted from its projInv in float64), so every field but
+    abi.VIEW_POSE_FIELDS is base's byte for byte.  prevMVP is the view's own viewProjMatrix (a static view)."""
+    proj = np.linalg.inv(np.asarray(base.projInv, np.float64).reshape(4, 4).T)
+    out = (abi.FrameInfo * len(views))()
+    for fi, view in zip(out, views):
+        C.memmove(C.addressof(fi), C.addressof(base), C.sizeof(abi.FrameInfo))
+        view = np.asarray(view, np.float64)
+        fi.viewMatrix[:] = _glm(view).tolist()
+        fi.viewInv[:] = _glm(np.linalg.inv(view)).tolist()
+        fi.viewProjMatrix[:] = _glm(proj @ view).tolist()
+        fi.prevMVP[:] = _glm(proj @ view).tolist()
+    return out
 
 
 def halton(index):

@@ -125,10 +125,10 @@ __device__ __forceinline__ void statAdd(unsigned long long* p, unsigned long lon
 // camera ray + sample start (samplePixel head: gltf_pathtrace.slang:502-530; getRay: pathtrace_functions.h.slang:791-811)
 // -------------------------------------------------------------------------------------------------
 // the pinhole or orthographic camera ray through pixel (x, y) + offset
-__device__ __forceinline__ void getRay(const FrameParams& F, uint32_t x, uint32_t y, float2 offset, float3& org, float3& dir)
+__device__ __forceinline__ void getRay(const FrameParams& F, const Camera& cam, uint32_t x, uint32_t y, float2 offset, float3& org, float3& dir)
 {
   const Mat4&  projI = *reinterpret_cast<const Mat4*>(F.fi.projInv);
-  const Mat4&  viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
+  const Mat4&  viewI = *reinterpret_cast<const Mat4*>(cam.viewInv);
   const float2 clip = f2(((float)x + offset.x) / F.fi.imageSize[0] * 2.0f - 1.0f, ((float)y + offset.y) / F.fi.imageSize[1] * 2.0f - 1.0f);
   float4       vc = mul_vM(f4(clip.x, clip.y, -1.0f, 1.0f), projI);
   vc = vc / vc.w;
@@ -147,11 +147,12 @@ __device__ __forceinline__ void getRay(const FrameParams& F, uint32_t x, uint32_
 __device__ void startSample(const PathState& P, const FrameParams& F, uint32_t i, uint32_t seed, float2 jitter, uint32_t sampleIdx)
 {
   const uint32_t px = pixelOf(F, i);
+  const Camera   cam = cameraOf(F, i);
   float3         org, dir;
-  getRay(F, px % (uint32_t)F.width, pixelRow(F, px), jitter, org, dir);
+  getRay(F, cam, px % (uint32_t)F.width, pixelRow(F, px), jitter, org, dir);
   if(!(F.fi.flags & B200PT_SCENE_IS_ORTHOGRAPHIC))
   {
-    const Mat4& viewI = *reinterpret_cast<const Mat4*>(F.fi.viewInv);
+    const Mat4& viewI = *reinterpret_cast<const Mat4*>(cam.viewInv);
     // thin-lens DOF: the two rand() are consumed even when aperture == 0 (:519-520)
     const float3 focalPoint = dir * F.pc.focalDistance;
     const float  cam_r1 = rnd(seed) * kTwoPi;
@@ -1296,13 +1297,16 @@ __global__ void __launch_bounds__(256) k_resolve(PathState P, DevScene S, const 
 
 // processPixel tail: mean over the frame's samples + running mean over frames (gltf_pathtrace.slang:596,619-630); on the
 // first frame also the NDC depth of the last sample's first hit (:600-616; Vulkan [0,1] range, 1 = far / miss).  A DLSS frame
-// replaces the image like a first frame (:619-622).
-__global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_constant__ FrameParams F, float4* __restrict__ accum, float* __restrict__ ndcDepth)
+// replaces the image like a first frame (:619-622).  With views, slot block v updates view v's image: view 0 is `accum` / `ndcDepth`,
+// view v > 0 starts at viewAccum / viewDepth + (v - 1) * pixels.
+__global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_constant__ FrameParams F, float4* __restrict__ accum, float* __restrict__ ndcDepth,
+                                                    float4* __restrict__ viewAccum, float* __restrict__ viewDepth)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
-  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels; i += stride)
+  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels * (uint32_t)F.views; i += stride)
   {
-    float4 img = f4(0.f, 0.f, 0.f, 0.f);
+    float4* const out = i < F.pixels ? accum + i : viewAccum + (i - F.pixels);
+    float4        img = f4(0.f, 0.f, 0.f, 0.f);
     // the frames of a batch are folded in frame order, each with the sample counts its own push constants would have carried
     for(int b = 0; b < F.batch; b++)
     {
@@ -1316,17 +1320,17 @@ __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_co
           float        d = 1.0f;
           if(fh.w > 0.0f)
           {
-            const Mat4&  vp = *reinterpret_cast<const Mat4*>(F.fi.viewProjMatrix);
+            const Mat4&  vp = *reinterpret_cast<const Mat4*>(cameraOf(F, i).viewProjMatrix);
             const float4 clip = mul_vM(f4(fh.x, fh.y, fh.z, 1.0f), vp);
             d = clip.z / clip.w;
           }
-          ndcDepth[i] = d;
+          *(i < F.pixels ? ndcDepth + i : viewDepth + (i - F.pixels)) = d;
         }
       }
       else
       {
         if(b == 0)
-          img = accum[i];
+          img = *out;
         const int    totalSamples = F.pc.totalSamples + b * F.pc.numSamples;
         const float  total = (float)totalSamples, n = (float)F.pc.numSamples;
         const float  after = (float)(totalSamples + F.pc.numSamples);
@@ -1334,7 +1338,7 @@ __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_co
         img = f4((old.x * total + c.x * n) / after, (old.y * total + c.y * n) / after, (old.z * total + c.z * n) / after, (old.w * total + c.w * n) / after);
       }
     }
-    accum[i] = img;
+    *out = img;
   }
 }
 
@@ -1369,7 +1373,7 @@ __global__ void __launch_bounds__(256) k_guide(PathState P, const __grid_constan
     if(n.w > 0.0f)
     {
       // mul(float3x3(viewMatrix), worldNormal) on the glm bytes (SURVEY.md section 8, convention note): M_glm^T * n
-      const float* m = F.fi.viewMatrix;
+      const float* m = cameraOf(F, slot).viewMatrix;
       camN = normalize(f3((m[0] * n.x + m[1] * n.y) + m[2] * n.z, (m[4] * n.x + m[5] * n.y) + m[6] * n.z, (m[8] * n.x + m[9] * n.y) + m[10] * n.z));
     }
     guide[i] = f4(a.x, a.y, a.z, __uint_as_float(compressUnitVec(camN)));
@@ -1397,8 +1401,9 @@ __global__ void __launch_bounds__(256) k_dlss_guides(PathState P, const __grid_c
     const uint32_t slot = i + (uint32_t)(F.batch - 1) * F.pixels;
     const float4   a = P.guideA[slot], n = P.guideN[slot];
     const bool     solid = P.pixSum[slot].w > 0.0f;  // sampleResult.radiance.w > 0 (the firefly clamp scales it by a positive factor)
+    const Camera         cam = cameraOf(F, slot);
     const DlssGuidePixel g = dlssPackGuides(xyz(a), f4(n.x, n.y, n.z, a.w), P.dlssSpec[slot], xyz(P.firstHit[slot]), xyz(P.prevHit[slot]), solid,
-                                            F.fi.viewProjMatrix, F.fi.prevMVP, f2(F.fi.imageSize[0], F.fi.imageSize[1]));
+                                            cam.viewProjMatrix, cam.prevMVP, f2(F.fi.imageSize[0], F.fi.imageSize[1]));
     out.albedo[i] = g.albedo;
     out.specAlbedo[i] = make_uint2((uint32_t)g.specAlbedo[0] | ((uint32_t)g.specAlbedo[1] << 16), (uint32_t)g.specAlbedo[2] | ((uint32_t)g.specAlbedo[3] << 16));
     out.normalRough[i] = make_uint2((uint32_t)g.normalRough[0] | ((uint32_t)g.normalRough[1] << 16), (uint32_t)g.normalRough[2] | ((uint32_t)g.normalRough[3] << 16));
@@ -1424,14 +1429,17 @@ __global__ void __launch_bounds__(256) k_snapshot_prev_transforms(const b200pt_r
 
 // traceSelectionRay (pathtrace_functions.h.slang:813-820) for every pixel of the first frame: the pixel-centre ray
 // (no jitter, no depth of field), IRaytracer::TraceLow semantics (raytracer_interface.h.slang:124-137: every triangle
-// opaque, no culling), object id = render node + 1, 0 on a miss.  One walk per thread; runs once per accumulation.
-__global__ void __launch_bounds__(128) k_select(DevScene S, const __grid_constant__ FrameParams F, uint32_t* __restrict__ objectId, DevStats* stats)
+// opaque, no culling), object id = render node + 1, 0 on a miss.  One walk per thread; runs once per accumulation.  With views, slot
+// block v writes view v's ids: view 0 to `objectId`, view v > 0 from viewIds + (v - 1) * pixels.
+__global__ void __launch_bounds__(128) k_select(DevScene S, const __grid_constant__ FrameParams F, uint32_t* __restrict__ objectId, uint32_t* __restrict__ viewIds,
+                                                DevStats* stats)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
-  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels; i += stride)
+  for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels * (uint32_t)F.views; i += stride)
   {
-    float3 org, dir;
-    getRay(F, i % (uint32_t)F.width, pixelRow(F, i), f2(0.5f, 0.5f), org, dir);
+    const uint32_t px = i % F.pixels;
+    float3         org, dir;
+    getRay(F, cameraOf(F, i), px % (uint32_t)F.width, pixelRow(F, px), f2(0.5f, 0.5f), org, dir);
     TravState T;
     uint2     stack[TravState::kStackSize];
     Cand      cand[1];
@@ -1441,7 +1449,7 @@ __global__ void __launch_bounds__(128) k_select(DevScene S, const __grid_constan
     }
     if(T.overflow)
       atomicOr(&stats->errorFlags, 1ull);
-    objectId[i] = (T.best.slot != 0xFFFFFFFFu) ? (S.triMeta[T.best.slot].x & 0x0fffffffu) + 1u : 0u;
+    *(i < F.pixels ? objectId + i : viewIds + (i - F.pixels)) = (T.best.slot != 0xFFFFFFFFu) ? (S.triMeta[T.best.slot].x & 0x0fffffffu) + 1u : 0u;
   }
 }
 
@@ -2117,6 +2125,7 @@ struct b200pt
     cudaEvent_t  done = nullptr;     // lane stream: all bounces of the lane's frame enqueued before it
     cudaEvent_t  freed = nullptr;    // main stream: k_accumulate has consumed the lane's pixSum
     bool         busy = false;       // `freed` has been recorded at least once since the pool was (re)built
+    ViewPose*    poses = nullptr;    // views > 1: the poses of the lane's frame (FrameParams::poses)
   };
   static constexpr int kMaxLanes = 8;
   Lane               lanes[kMaxLanes];
@@ -2127,6 +2136,12 @@ struct b200pt
   int                   pendingCount = 0;
   b200pt_frame_info     pendingFi{};
   b200pt_push_constant  pendingPc{};  // the FIRST pending frame's constants
+  // views (b200pt_set_views / b200pt_render_views): `views` camera poses of one frame run as one wavefront of views x pixels paths,
+  // each into its own images.  View 0 is dAccum / dSelect / dNdcDepth; views 1.. are (views - 1) x pixels images in poolMem.
+  int                   views = 1;
+  float4*               dViewAccum = nullptr;
+  uint32_t*             dViewSelect = nullptr;
+  float*                dViewDepth = nullptr;
   int                numLanes = 4;   // frames in flight (b200pt_set_frames_in_flight)
   uint64_t           frameSerial = 0;
   int                lastLane = -1;
@@ -2379,10 +2394,14 @@ void freePool(b200pt* h)
   h->dTonemapped = nullptr;
   h->dGuide = nullptr;
   h->dDlss = nullptr;
+  h->dViewAccum = nullptr;
+  h->dViewSelect = nullptr;
+  h->dViewDepth = nullptr;
   h->numPaths = 0;
   for(int l = 0; l < b200pt::kMaxLanes; l++)
   {
     h->lanes[l].P = PathState{};
+    h->lanes[l].poses = nullptr;
     for(int k = 0; k < 6; k++)
       h->lanes[l].dQ[k] = nullptr;
   }
@@ -2612,7 +2631,7 @@ void launchSort(const Launcher& ctx, const b200pt::Lane& L, const uint32_t* q, c
 
 }  // namespace
 extern "C" {
-static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count);
+static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count, const b200pt_frame_info* viewFis = nullptr);
 static int flushPending(b200pt_t* h);
 }
 namespace {
@@ -4487,17 +4506,20 @@ int b200pt_resize(b200pt_t* h, int width, int height, int tile_y0, int tile_rows
     return rc;
   freePool(h);
   const size_t n = (size_t)width * tile_rows;          // pixels of the tile: image-sized buffers
-  const size_t nPool = n * (size_t)std::max(h->batch, 1);  // path slots per lane
+  const size_t nPool = n * (size_t)std::max(h->batch, h->views);  // path slots per lane (at most one of the two is above 1)
   // nothing of the handle's geometry is committed before every allocation has succeeded: a failed resize leaves
   // numPaths == 0 and null pointers, so later calls fail their guards instead of touching freed memory
   DeviceArena A;
   PathState   P[b200pt::kMaxLanes];
   uint32_t*   dQ[b200pt::kMaxLanes][6] = {};
+  ViewPose*   poses[b200pt::kMaxLanes] = {};
   for(int l = 0; l < h->numLanes; l++)
   {
     allocPathState(h, A, nPool, P[l]);
     for(int k = 0; k < 6; k++)
       dQ[l][k] = A.alloc<uint32_t>(nPool);
+    if(h->views > 1)
+      poses[l] = A.alloc<ViewPose>((size_t)h->views);
   }
   if(!A.ok())
     return failed(h, A, "path pool");
@@ -4520,10 +4542,19 @@ int b200pt_resize(b200pt_t* h, int width, int height, int tile_y0, int tile_rows
   uchar4* const tonemapped = A.alloc<uchar4>(n);
   if(!tonemapped)
     return failed(h, A, "tonemapped image");
+  const size_t    nv = n * (size_t)(h->views - 1);  // pixels of views 1..
+  float4* const   viewAccum = nv ? A.alloc<float4>(nv) : nullptr;
+  uint32_t* const viewSelect = nv ? A.alloc<uint32_t>(nv) : nullptr;
+  float* const    viewDepth = nv ? A.alloc<float>(nv) : nullptr;
+  if(nv && !A.ok())
+    return failed(h, A, "view images");
   const cudaStream_t st = h->stream;
   if((guide && cudaMemsetAsync(guide, 0, n * 16, st) != cudaSuccess) || (dlss && cudaMemsetAsync(dlss, 0, dlssBytes, st) != cudaSuccess)
      || cudaMemsetAsync(select, 0, n * 4, st) != cudaSuccess || cudaMemsetAsync(ndcDepth, 0, n * 4, st) != cudaSuccess
-     || cudaMemsetAsync(accum, 0, n * 16, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+     || cudaMemsetAsync(accum, 0, n * 16, st) != cudaSuccess
+     || (nv && (cudaMemsetAsync(viewAccum, 0, nv * 16, st) != cudaSuccess || cudaMemsetAsync(viewSelect, 0, nv * 4, st) != cudaSuccess
+                || cudaMemsetAsync(viewDepth, 0, nv * 4, st) != cudaSuccess))
+     || cudaStreamSynchronize(st) != cudaSuccess)
   {
     h->err = "b200pt_resize: clearing the new images failed";
     return B200PT_E_CUDA;
@@ -4533,7 +4564,11 @@ int b200pt_resize(b200pt_t* h, int width, int height, int tile_y0, int tile_rows
   {
     h->lanes[l].P = P[l];
     std::copy(dQ[l], dQ[l] + 6, h->lanes[l].dQ);
+    h->lanes[l].poses = poses[l];
   }
+  h->dViewAccum = viewAccum;
+  h->dViewSelect = viewSelect;
+  h->dViewDepth = viewDepth;
   h->dAccumOwned = accum;
   h->dSelect = select;
   h->dNdcDepth = ndcDepth;
@@ -4867,6 +4902,11 @@ int b200pt_set_frame_batch(b200pt_t* h, int n)
     return B200PT_E_INVALID;
   if(n == h->batch)
     return B200PT_OK;
+  if(n > 1 && h->views > 1)
+  {
+    h->err = "b200pt_set_frame_batch: frames are not batched while more than one view is set (b200pt_set_views)";
+    return B200PT_E_UNSUPPORTED;
+  }
   if(const int rc = enter(h, false))
     return rc;
   h->batch = n;
@@ -4895,45 +4935,54 @@ int b200pt_set_profiling(b200pt_t* h, int enabled)
   return B200PT_OK;
 }
 
-int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc)
+// the checks every rendered frame passes (`who` names the entry point in the error)
+static int checkFrame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, const char* who)
 {
-  if(!h || !fi || !pc)
-    return B200PT_E_INVALID;
+  const std::string name(who);
   if(!h->haveScene || h->numPaths == 0)
   {
-    h->err = "b200pt_render_frame: set_scene and resize must come first";
+    h->err = name + ": set_scene and resize must come first";
     return B200PT_E_INVALID;
   }
   if(!(fi->flags & B200PT_SCENE_USE_HDR_ENVIRONMENT) || !h->haveEnv)
   {
-    h->err = "b200pt_render_frame: only the HDR environment (--envSystem 1) is built; physical sky is out of scope";
+    h->err = name + ": only the HDR environment (--envSystem 1) is built; physical sky is out of scope";
     return B200PT_E_UNSUPPORTED;
   }
   if((fi->flags & B200PT_SCENE_USE_HDR_ENVIRONMENT) && fi->envBlur > 0.0f && !(fi->flags & B200PT_SCENE_USE_SOLID_BACKGROUND))
   {
-    h->err = "b200pt_render_frame: the blurred HDR backplate (envBlur > 0: nvshaders' smoothHDRBlur, external) is not built";
+    h->err = name + ": the blurred HDR backplate (envBlur > 0: nvshaders' smoothHDRBlur, external) is not built";
     return B200PT_E_UNSUPPORTED;
   }
   if((pc->flags & B200PT_PT_USE_DLSS) && !h->dlss)
   {
-    h->err = "b200pt_render_frame: ePtUseDlss needs the DLSS guide images (b200pt_set_dlss_guides(h, 1) first)";
+    h->err = name + ": ePtUseDlss needs the DLSS guide images (b200pt_set_dlss_guides(h, 1) first)";
     return B200PT_E_INVALID;
   }
   if((pc->flags & B200PT_PT_USE_DLSS) && pc->numSamples != 1)
   {
-    h->err = "b200pt_render_frame: the DLSS variant renders one sample per frame (numSamples must be 1)";
+    h->err = name + ": the DLSS variant renders one sample per frame (numSamples must be 1)";
     return B200PT_E_INVALID;
   }
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && !h->guides)
   {
-    h->err = "b200pt_render_frame: ePtUseOptixDenoiser needs the guide image (b200pt_set_guide_outputs(h, 1) first)";
+    h->err = name + ": ePtUseOptixDenoiser needs the guide image (b200pt_set_guide_outputs(h, 1) first)";
     return B200PT_E_INVALID;
   }
   if(pc->numSamples < 1 || pc->maxDepth < 0 || (int)fi->imageSize[0] != h->width || (int)fi->imageSize[1] != h->height)
   {
-    h->err = "b200pt_render_frame: bad numSamples / maxDepth / imageSize";
+    h->err = name + ": bad numSamples / maxDepth / imageSize";
     return B200PT_E_INVALID;
   }
+  return B200PT_OK;
+}
+
+int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc)
+{
+  if(!h || !fi || !pc)
+    return B200PT_E_INVALID;
+  if(const int rc = checkFrame(h, fi, pc, "b200pt_render_frame"))
+    return rc;
   if(h->batch <= 1)
     return launchFrames(h, fi, pc, 1);
   if(pc->flags & B200PT_PT_USE_DLSS)
@@ -4971,6 +5020,109 @@ int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   return B200PT_OK;
 }
 
+int b200pt_set_views(b200pt_t* h, int n)
+{
+  if(!h || n < 1 || n > 64)
+    return B200PT_E_INVALID;
+  if(n == h->views)
+    return B200PT_OK;
+  if(n > 1 && h->batch > 1)
+  {
+    h->err = "b200pt_set_views: more than one view needs frame batching off (b200pt_set_frame_batch(h, 1))";
+    return B200PT_E_UNSUPPORTED;
+  }
+  if(const int rc = enter(h, false))
+    return rc;
+  const int old = h->views;
+  h->views = n;
+  const int rc = rebuildPool(h);
+  if(rc)
+    h->views = old;  // like a failed b200pt_resize the handle has no pool now; the next resize builds it for the old count
+  return rc;
+}
+
+int b200pt_render_views(b200pt_t* h, const b200pt_frame_info* fis, uint32_t n, const b200pt_push_constant* pc)
+{
+  if(!h || !fis || !pc)
+    return B200PT_E_INVALID;
+  if(n != (uint32_t)h->views)
+  {
+    h->err = "b200pt_render_views: n must equal the view count of b200pt_set_views";
+    return B200PT_E_INVALID;
+  }
+  // the views share every field but the pose: fis[v] with fis[0]'s pose must be fis[0], byte for byte
+  for(uint32_t v = 1; v < n; v++)
+  {
+    b200pt_frame_info a = fis[v];
+    memcpy(a.viewMatrix, fis[0].viewMatrix, sizeof(a.viewMatrix));
+    memcpy(a.viewInv, fis[0].viewInv, sizeof(a.viewInv));
+    memcpy(a.viewProjMatrix, fis[0].viewProjMatrix, sizeof(a.viewProjMatrix));
+    memcpy(a.prevMVP, fis[0].prevMVP, sizeof(a.prevMVP));
+    if(memcmp(&a, &fis[0], sizeof(a)) != 0)
+    {
+      h->err = "b200pt_render_views: view " + std::to_string(v) + " differs from view 0 in a field other than viewMatrix, viewInv, viewProjMatrix and prevMVP";
+      return B200PT_E_INVALID;
+    }
+  }
+  if(n > 1 && (pc->flags & (B200PT_PT_USE_DLSS | B200PT_PT_USE_OPTIX_DENOISER)))
+  {
+    h->err = "b200pt_render_views: the DLSS and OptiX-denoiser guide images belong to one displayed frame; render them with b200pt_render_frame";
+    return B200PT_E_UNSUPPORTED;
+  }
+  if(const int rc = checkFrame(h, &fis[0], pc, "b200pt_render_views"))
+    return rc;
+  if(const int rc = flushPending(h))
+    return rc;
+  return launchFrames(h, &fis[0], pc, 1, n > 1 ? fis : nullptr);
+}
+
+// view 0 is the handle's accumulation, selection and depth images; view v > 0 sits at (v - 1) x pixels in the view images
+static void viewImages(b200pt_t* h, uint32_t view, float4** rgba, uint32_t** ids, float** depth)
+{
+  const size_t off = view ? (size_t)(view - 1) * h->numPaths : 0;
+  *rgba = view ? h->dViewAccum + off : h->dAccum;
+  *ids = view ? h->dViewSelect + off : h->dSelect;
+  *depth = view ? h->dViewDepth + off : h->dNdcDepth;
+}
+
+int b200pt_read_views(b200pt_t* h, uint32_t view, float* host_rgba32f, uint32_t* host_object_ids, float* host_ndc_depth, size_t num_pixels)
+{
+  if(!h || h->numPaths == 0 || view >= (uint32_t)h->views || num_pixels < (size_t)h->numPaths)
+    return B200PT_E_INVALID;
+  if(const int rc = enter(h, false))
+    return rc;
+  float4*   rgba;
+  uint32_t* ids;
+  float*    depth;
+  viewImages(h, view, &rgba, &ids, &depth);
+  const size_t n = h->numPaths;
+  if(host_rgba32f)
+    CK(cudaMemcpyAsync(host_rgba32f, rgba, n * 16, cudaMemcpyDeviceToHost, h->stream));
+  if(host_object_ids)
+    CK(cudaMemcpyAsync(host_object_ids, ids, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  if(host_ndc_depth)
+    CK(cudaMemcpyAsync(host_ndc_depth, depth, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return B200PT_OK;
+}
+
+int b200pt_get_views_device(b200pt_t* h, uint32_t view, float** dev_rgba32f, uint32_t** dev_object_ids, float** dev_ndc_depth)
+{
+  if(!h || h->numPaths == 0 || view >= (uint32_t)h->views)
+    return B200PT_E_INVALID;
+  float4*   rgba;
+  uint32_t* ids;
+  float*    depth;
+  viewImages(h, view, &rgba, &ids, &depth);
+  if(dev_rgba32f)
+    *dev_rgba32f = reinterpret_cast<float*>(rgba);
+  if(dev_object_ids)
+    *dev_object_ids = ids;
+  if(dev_ndc_depth)
+    *dev_ndc_depth = depth;
+  return B200PT_OK;
+}
+
 static int flushPending(b200pt_t* h)
 {
   if(h->pendingCount == 0)
@@ -4987,8 +5139,9 @@ int b200pt_flush(b200pt_t* h)
   return flushPending(h);
 }
 
-// enqueues the launch chain of `count` consecutive frames (count > 1: one batched wavefront, FrameParams::batch)
-static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count)
+// enqueues the launch chain of `count` consecutive frames (count > 1: one batched wavefront, FrameParams::batch), or with viewFis
+// (count 1) of the handle's views, whose poses replace fi's (FrameParams::views)
+static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count, const b200pt_frame_info* viewFis)
 {
   CK(cudaSetDevice(h->device));
   FrameParams F;
@@ -5003,7 +5156,9 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   F.bandRank = h->bandRank;
   F.pixels = h->numPaths;
   F.batch = count;
-  F.numPaths = h->numPaths * (uint32_t)count;
+  F.views = viewFis ? h->views : 1;
+  F.poses = nullptr;
+  F.numPaths = h->numPaths * (uint32_t)count * (uint32_t)F.views;
   F.prevObjectToWorld = ((pc->flags & B200PT_PT_USE_DLSS) && h->prevO2WValid) ? h->dPrevO2W : nullptr;
   h->prevO2WValid = false;
   h->renderedSinceUpdate = true;
@@ -5016,6 +5171,20 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
     CK(cudaStreamWaitEvent(L.stream, L.freed, 0));
   if(h->profiling && h->lastLane >= 0 && h->lastLane != laneIdx)
     CK(cudaStreamWaitEvent(L.stream, h->lanes[h->lastLane].freed, 0));
+  if(F.views > 1)
+  {
+    // on the lane's stream, behind the wait: the lane's previous frame has read its poses
+    std::vector<ViewPose> poses((size_t)F.views);
+    for(int v = 0; v < F.views; v++)
+    {
+      memcpy(poses[v].viewMatrix, viewFis[v].viewMatrix, sizeof(poses[v].viewMatrix));
+      memcpy(poses[v].viewInv, viewFis[v].viewInv, sizeof(poses[v].viewInv));
+      memcpy(poses[v].viewProjMatrix, viewFis[v].viewProjMatrix, sizeof(poses[v].viewProjMatrix));
+      memcpy(poses[v].prevMVP, viewFis[v].prevMVP, sizeof(poses[v].prevMVP));
+    }
+    CK(cudaMemcpyAsync(L.poses, poses.data(), poses.size() * sizeof(ViewPose), cudaMemcpyHostToDevice, L.stream));
+    F.poses = L.poses;
+  }
   const Counters C{L.dCounters, kMaxIters};
   CK(cudaMemsetAsync(L.dCounters, 0, sizeof(uint32_t) * kCounterArrays * kMaxIters, L.stream));
   Launcher ctx{h, L.stream, laneIdx, h->frameSerial - 1, -1, h->profiling || h->timeline != nullptr, F.numPaths};
@@ -5077,8 +5246,8 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   ctx.stream = h->stream;
   ctx.lane = -1;
   if(pc->flags & B200PT_PT_FIRST_FRAME)
-    ctx(kStageOther, [&](cudaStream_t st) { k_select<<<gridWide, 128, 0, st>>>(h->S, F, h->dSelect, h->dStats); });
-  ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth); });
+    ctx(kStageOther, [&](cudaStream_t st) { k_select<<<gridWide, 128, 0, st>>>(h->S, F, h->dSelect, h->dViewSelect, h->dStats); });
+  ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth, h->dViewAccum, h->dViewDepth); });
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && h->dGuide)
     ctx(kStageOther, [&](cudaStream_t st) { k_guide<<<gridWide, 256, 0, st>>>(L.P, F, h->dGuide); });
   if((pc->flags & B200PT_PT_USE_DLSS) && h->dDlss)

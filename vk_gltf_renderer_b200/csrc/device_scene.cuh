@@ -165,6 +165,12 @@ struct DevScene
   int                          envW, envH;
 };
 
+// the fields of b200pt_frame_info in which the views of one b200pt_render_views call may differ
+struct ViewPose
+{
+  float viewMatrix[16], viewInv[16], viewProjMatrix[16], prevMVP[16];
+};
+
 struct FrameParams
 {
   b200pt_frame_info    fi;
@@ -178,13 +184,32 @@ struct FrameParams
   // frameCount and b * numSamples to totalSamples (what the host loop would have passed, src/renderer_pathtracer.cpp:1496-1574).
   uint32_t             pixels;    // tileRows * width
   int                  batch;     // >= 1
+  // Views (b200pt_render_views): `views` camera poses of ONE frame run as one wavefront.  Slot i belongs to pixel i % pixels of
+  // view i / pixels; every view shares the frame's constants except its pose, poses[v].  At most one of batch and views is above 1.
+  int                  views;     // >= 1
+  const ViewPose*      poses;     // views > 1: one per view, on the device
   // DLSS frames: objectToWorld of every render node as the previous frame saw it (16 floats each, glm order), or null when no
   // transform changed since that frame (pushConst.prevRenderNodeObjectToWorld, src/renderer_pathtracer.cpp:1553-1561)
   const float*         prevObjectToWorld;
 };
 
-PT_D uint32_t pixelOf(const FrameParams& F, uint32_t i) { return F.batch > 1 ? i % F.pixels : i; }
+// the camera of a path slot: its view's pose, or F.fi's with one view
+struct Camera
+{
+  const float *viewMatrix, *viewInv, *viewProjMatrix, *prevMVP;
+};
+
+PT_D uint32_t pixelOf(const FrameParams& F, uint32_t i) { return F.batch > 1 || F.views > 1 ? i % F.pixels : i; }
 PT_D uint32_t frameOf(const FrameParams& F, uint32_t i) { return F.batch > 1 ? i / F.pixels : 0u; }
+PT_D Camera   cameraOf(const FrameParams& F, uint32_t i)
+{
+  if(F.views > 1)
+  {
+    const ViewPose& v = F.poses[i / F.pixels];
+    return {v.viewMatrix, v.viewInv, v.viewProjMatrix, v.prevMVP};
+  }
+  return {F.fi.viewMatrix, F.fi.viewInv, F.fi.viewProjMatrix, F.fi.prevMVP};
+}
 // the slot renders the first frame of an accumulation (its sample overwrites the image, frame-0 outputs are written)
 PT_D bool isFirstFrame(const FrameParams& F, uint32_t i) { return (F.pc.flags & B200PT_PT_FIRST_FRAME) != 0 && (F.batch <= 1 || i < F.pixels); }
 

@@ -552,6 +552,25 @@ void PathTracer::setFrameBatch(int n) { check(b200pt_set_frame_batch(m_h, n), "b
 
 void PathTracer::flush() { check(b200pt_flush(m_h), "b200pt_flush"); }
 
+void PathTracer::setViews(int n) { check(b200pt_set_views(m_h, n), "b200pt_set_views"); }
+
+void PathTracer::renderViews(const std::vector<b200pt_frame_info>& fis, const b200pt_push_constant& pc)
+{
+  check(b200pt_render_views(m_h, fis.data(), (uint32_t)fis.size(), &pc), "b200pt_render_views");
+}
+
+std::vector<float> PathTracer::readView(uint32_t view, std::vector<uint32_t>* objectIds, std::vector<float>* ndcDepth)
+{
+  const size_t       n = (size_t)m_width * m_tileRows;
+  std::vector<float> rgba(n * 4);
+  if(objectIds)
+    objectIds->resize(n);
+  if(ndcDepth)
+    ndcDepth->resize(n);
+  check(b200pt_read_views(m_h, view, rgba.data(), objectIds ? objectIds->data() : nullptr, ndcDepth ? ndcDepth->data() : nullptr, n), "b200pt_read_views");
+  return rgba;
+}
+
 b200pt_stats PathTracer::stats()
 {
   b200pt_stats s{};

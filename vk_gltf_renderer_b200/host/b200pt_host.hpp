@@ -167,6 +167,11 @@ public:
   void               setFramesInFlight(int n);
   void               setFrameBatch(int n);  // b200pt_set_frame_batch
   void               flush();               // b200pt_flush
+  // views (b200pt_set_views / b200pt_render_views): n poses of one frame as one wavefront, each into its own images; readView(v) is
+  // view v's RGBA32F image of this tile, with its object ids and NDC depth when asked for
+  void               setViews(int n);
+  void               renderViews(const std::vector<b200pt_frame_info>& fis, const b200pt_push_constant& pc);
+  std::vector<float> readView(uint32_t view, std::vector<uint32_t>* objectIds = nullptr, std::vector<float>* ndcDepth = nullptr);
   b200pt_stats       stats();
   void               resetStats();
   b200pt_t*          handle() { return m_h; }

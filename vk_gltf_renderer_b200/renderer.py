@@ -427,6 +427,35 @@ class PathTracer:
     def flush(self):
         self._ck(self._L.b200pt_flush(self._h), "b200pt_flush")
 
+    def set_views(self, n):
+        """render n camera poses of one frame as one wavefront, each into its own images (include/b200pt.h); clears the images"""
+        self._ck(self._L.b200pt_set_views(self._h, n), "b200pt_set_views")
+        self._views = n
+
+    def render_views(self, fis, pc):
+        """one frame of every view: fis is a sequence of FrameInfo that differ only in their pose (camera.view_frame_infos)"""
+        arr = fis if isinstance(fis, C.Array) else (abi.FrameInfo * len(fis))(*fis)
+        self._ck(self._L.b200pt_render_views(self._h, arr, len(arr), C.byref(pc)), "b200pt_render_views")
+
+    def read_views(self):
+        """every view's images: RGBA32F [V, rows, W, 4], object ids uint32 [V, rows, W] and NDC depth float32 [V, rows, W]"""
+        w, _ = self._size
+        rows = self._tile[1]
+        v = getattr(self, "_views", 1)
+        rgba = np.empty((v, rows, w, 4), np.float32)
+        ids = np.empty((v, rows, w), np.uint32)
+        depth = np.empty((v, rows, w), np.float32)
+        for k in range(v):
+            self._ck(self._L.b200pt_read_views(self._h, k, rgba[k].ctypes.data_as(C.c_void_p), ids[k].ctypes.data_as(C.c_void_p),
+                                               depth[k].ctypes.data_as(C.c_void_p), rows * w), "b200pt_read_views")
+        return rgba, ids, depth
+
+    def views_device_ptrs(self, view):
+        """device pointers of one view's RGBA32F, object-id and depth images"""
+        rgba, ids, depth = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self._ck(self._L.b200pt_get_views_device(self._h, view, C.byref(rgba), C.byref(ids), C.byref(depth)), "b200pt_get_views_device")
+        return rgba.value, ids.value, depth.value
+
     def accum_device_ptr(self):
         p, n = C.c_void_p(), C.c_size_t()
         self._ck(self._L.b200pt_get_accum_device(self._h, C.byref(p), C.byref(n)), "b200pt_get_accum_device")
