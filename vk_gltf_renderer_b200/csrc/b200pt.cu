@@ -336,6 +336,29 @@ __device__ __forceinline__ void walkQueue(const uint32_t* __restrict__ q, uint32
     atomicAdd(MODE == 1 ? &stats->closestRays : &stats->shadowRays, (unsigned long long)count);
 }
 
+// is every one of the n candidates a cap or a hole (tagged by the CAPS walk)?
+__device__ __forceinline__ bool knownOpacities(const Cand* cand, int n)
+{
+  bool known = true;
+#pragma unroll
+  for(int i = 0; i < kCand; i++)
+    if(i < n)
+      known &= (cand[i * kWalkBlock].slot & (kCandCap | kCandHole)) != 0;
+  return known;
+}
+// the first n candidates into the path state for k_alpha (a CAPS walk's tags cleared)
+template <bool CAPS>
+__device__ __forceinline__ void writeCandidates(const PathState& P, uint32_t path, const Cand* cand, int n)
+{
+#pragma unroll
+  for(int i = 0; i < kCand; i++)
+    if(i < n)
+    {
+      const Cand c = cand[i * kWalkBlock];
+      P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(CAPS ? c.slot & kCandSlot : c.slot));
+    }
+}
+
 // IRaytracer::Trace, geometry part, for every path in the queue: ONE walk of the scene tree gives the closest
 // FORCE_OPAQUE hit and the kCand nearest any-hit candidates in front of it (traverse.cuh).  The stochastic alpha
 // tests need textures and touch only the few lanes whose walk just ended -- inside this kernel they ran with ~2 of
@@ -373,13 +396,31 @@ __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_trace(PathState 
     const int n = T.candidatesInFront(cand, kWalkBlock);
     if(n > 0)
     {
+      // every candidate a cap or a hole (alpha_caps.cuh): its opacity is exactly 1 or 0, so the draws alone decide the any-hit loop of
+      // k_alpha<false> and it runs here, without texels -- unless all kCand were rejected and a continuation round must follow
+      if(CAPS && knownOpacities(cand, n))
+      {
+        uint32_t* const seedOut = reinterpret_cast<uint32_t*>(&P.misc[path]) + 3;
+        uint32_t        seed = *seedOut;
+        int             acc = -1;
 #pragma unroll
-      for(int i = 0; i < kCand; i++)
-        if(i < n)
+        for(int i = 0; i < kCand; i++)
+          if(i < n && acc < 0 && rnd(seed) <= ((cand[i * kWalkBlock].slot & kCandCap) ? 1.0f : 0.0f))
+            acc = i;
+        if(acc >= 0 || n < kCand)
         {
-          const Cand c = cand[i * kWalkBlock];
-          P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
+          if(acc >= 0)
+          {
+            const Cand     c = cand[acc * kWalkBlock];
+            const uint32_t slot = c.slot & kCandSlot;
+            const bool     flip = ((__float_as_uint(__ldg(&S.bvh.tris[slot * 3 + 0]).w) >> 28) & TRI_FLIPPED) != 0;
+            P.hit[path] = f4(c.t, flip ? c.v : c.u, flip ? c.u : c.v, __uint_as_float(slot));
+          }
+          *seedOut = seed;
+          return true;
         }
+      }
+      writeCandidates<CAPS>(P, path, cand, n);
       P.candInfo[path] = make_uint2((uint32_t)n, cand[(n - 1) * kWalkBlock].gid);
       queuePush(qAlpha, cntAlpha, (uint32_t)path);
     }
@@ -1161,14 +1202,28 @@ __global__ void __launch_bounds__(kWalkBlock, kWalkCtasPerSM) k_shadow(PathState
     else
     {
       const int n = T.collectN;
-#pragma unroll
-      for(int i = 0; i < kCand; i++)
-        if(i < n)
-        {
-          const Cand c = cand[i * kWalkBlock];
-          P.cand[i][path] = f4(c.t, c.u, c.v, __uint_as_float(c.slot));
-        }
       info = make_uint2((uint32_t)n, n > 0 ? cand[(n - 1) * kWalkBlock].gid : 0u);
+      // every candidate a cap (opacity 1, transmission <= 0.01: it blocks the ray) or a hole (opacity 0: never passes): k_alpha<true>'s
+      // loop here, without texels, in a ray's first round (a continuation round folds the transmission parked by the previous one)
+      if(CAPS && !cont && n > 0 && knownOpacities(cand, n))
+      {
+        uint32_t* const seedOut = reinterpret_cast<uint32_t*>(&P.misc[path]) + 3;
+        uint32_t        seed = *seedOut;
+        bool            blocked = false;
+#pragma unroll
+        for(int i = 0; i < kCand; i++)
+          if(i < n && !blocked && rnd(seed) < ((cand[i * kWalkBlock].slot & kCandCap) ? 1.0f : 0.0f))
+            blocked = true;
+        if(blocked || n < kCand)
+        {
+          const float4 c = P.shC[path];
+          P.shC[path] = f4(xyz(c) * (blocked ? f3(0.0f) : f3(1.0f)), c.w);
+          *seedOut = seed;
+          P.candInfo[path] = info;
+          return true;
+        }
+      }
+      writeCandidates<CAPS>(P, path, cand, n);
     }
     P.candInfo[path] = info;
     // (a continuation path always goes back to k_alpha: its running transmission is parked and must be folded)
@@ -1631,8 +1686,9 @@ __global__ void __launch_bounds__(256) k_gather_alpha(AlphaRec* recs, const uint
   }
 }
 
-// the alpha caps of the alpha records (alpha_caps.cuh), one thread per (record, grid cell of kCapLevel): the cap micro-triangles of
-// record r are OR-ed into bits[r * kCapWords ...] (zeroed by the caller); shadowOk[r]: the record's material may cap a shadow ray
+// the alpha caps and holes of the alpha records (alpha_caps.cuh), one thread per (record, grid cell of kCapLevel): the cap
+// micro-triangles of record r are OR-ed into bits[r * 2 * kCapWords ...], its holes into the kCapWords words behind them (zeroed by the
+// caller); shadowOk[r]: the record's material may cap a shadow ray
 #pragma nv_exec_check_disable
 __global__ void __launch_bounds__(256) k_cap_bake(const AlphaRec* __restrict__ recs, uint32_t n, uint32_t* bits, uint8_t* shadowOk)
 {
@@ -1648,8 +1704,9 @@ __global__ void __launch_bounds__(256) k_cap_bake(const AlphaRec* __restrict__ r
     auto      alpha8 = [&](int x, int y) { return (int)__ldg(r.lv0 + (((y >> 2) * tpr + (x >> 2)) << 4) + ((y & 3) << 2) + (x & 3)).w; };
     auto      wrap = [](int i, int m, int mode) { return wrapFast(i, m, mode); };
     uint32_t  idx;
-    if(capBakeCell(k, r.uv, r.w0, r.h0, r.wrap, r.factor, r.cutoff, r.modeFlags, r.colA, r.lv0 != nullptr, alpha8, wrap, idx))
-      atomicOr(&bits[(size_t)rec * kCapWords + (idx >> 5)], 1u << (idx & 31u));
+    bool      cap, hole;
+    if(capBakeCell(k, r.uv, r.w0, r.h0, r.wrap, r.factor, r.cutoff, r.modeFlags, r.colA, r.lv0 != nullptr, alpha8, wrap, idx, cap, hole) && (cap || hole))
+      atomicOr(&bits[(size_t)rec * 2 * kCapWords + (hole ? kCapWords : 0u) + (idx >> 5)], 1u << (idx & 31u));
   }
 }
 
@@ -3567,12 +3624,13 @@ void setTreeWindow(b200pt* h)
   }
 }
 
-// The alpha caps (alpha_caps.cuh) of the handle's scene, baked from its alpha records into h->capMem: the reference words of the
-// closest-hit tree and of the shadow rays' triangle array, and the bit maps of the triangles that have both cap and non-cap
-// micro-triangles.  Called after every change of the alpha records (b200pt_set_scene, a scene edit that changed an alpha input, a
-// rebuild).  Scenes with opacity micromaps or without non-opaque triangles get none, and so does every scene while
-// B200PT_ALPHA_CAPS=0 (caps change no result: the switch lets the tests compare walks with and without them).  The records are baked
-// kChunk at a time, so the unpacked maps in flight stay at kChunk x 128 B on the device and on the host whatever the scene's size.
+// The alpha caps and holes (alpha_caps.cuh) of the handle's scene, baked from its alpha records into h->capMem: the reference words of
+// the closest-hit tree and of the shadow rays' triangle array, and the maps of the triangles whose micro-triangles are not all of one
+// kind.  Called after every change of the alpha records (b200pt_set_scene, a scene edit that changed an alpha input, a rebuild): a
+// stale map would skip texels that are no longer transparent or end walks at texels that are no longer opaque.  Scenes with opacity
+// micromaps or without non-opaque triangles get none, and so does every scene while B200PT_ALPHA_CAPS=0 (caps and holes change no
+// result: the switch lets the tests compare walks with and without them).  The records are baked kChunk at a time, so the unpacked
+// maps in flight stay at kChunk x 256 B on the device and on the host whatever the scene's size.
 // Returns an error code with h->err set on a failure; the handle is then left without caps.
 int bakeAlphaCaps(b200pt* h)
 {
@@ -3583,44 +3641,54 @@ int bakeAlphaCaps(b200pt* h)
   const char* e = getenv("B200PT_ALPHA_CAPS");
   if(!S.hasAlpha || S.bvh.ommRef || !h->dAlphaRecsW || (e && atoi(e) == 0))
     return B200PT_OK;
-  constexpr uint32_t kChunk = 1u << 16;
+  constexpr uint32_t kChunk = 1u << 16, kMapWords = 2 * kCapWords;
   const cudaStream_t st = h->stream;
   const uint32_t     nC = h->tree[0].numTriSlots, nS = h->tree[1].numTriSlots, base = S.alphaBaseS, nA = nS - base;
+  if(nC >= kCandCapsSlots || nS >= kCandCapsSlots)
+    return B200PT_OK;  // (the walks tag caps and holes in a candidate's slot bits)
   DeviceArena        scratch;
-  uint32_t* const    dBits = scratch.alloc<uint32_t>((size_t)std::min(nA, kChunk) * kCapWords);
+  uint32_t* const    dBits = scratch.alloc<uint32_t>((size_t)std::min(nA, kChunk) * kMapWords);
   uint8_t* const     dShadowOk = scratch.alloc<uint8_t>(std::min(nA, kChunk));
   if(!scratch.ok())
     return failed(h, scratch, "alpha caps");
-  // per record: no cap, all caps, or its map appended to the packed bits
-  std::vector<uint32_t> refOfRec(nA, kCapNone), packed, bits((size_t)std::min(nA, kChunk) * kCapWords);
+  // per record and ray kind (closest-hit rays, shadow rays: no caps unless shadowOk): neither, all caps, all holes, or its map
+  // appended to the packed maps
+  std::vector<uint32_t> refOfRec(nA, kCapNone), refOfRecS(nA, kCapNone), packed, bits((size_t)std::min(nA, kChunk) * kMapWords);
   std::vector<uint8_t>  shadowOk(nA);
   bool                  any = false;
+  auto                  refOf = [&](const uint32_t* m, bool capsToo) {
+    uint32_t caps = 0, holes = 0;
+    for(uint32_t w = 0; w < kCapWords; w++)
+    {
+      caps += capsToo ? (uint32_t)__builtin_popcount(m[w]) : 0u;
+      holes += (uint32_t)__builtin_popcount(m[kCapWords + w]);
+    }
+    if(caps == 0 && holes == 0)
+      return kCapNone;
+    any = true;
+    if(caps == kCapMicro || holes == kCapMicro)
+      return caps ? kCapAll : kHoleAll;
+    const uint32_t ref = (uint32_t)packed.size();
+    packed.insert(packed.end(), m, m + kMapWords);
+    if(!capsToo)
+      std::fill(packed.begin() + ref, packed.begin() + ref + kCapWords, 0u);
+    return ref;
+  };
   for(uint32_t r0 = 0; r0 < nA; r0 += kChunk)
   {
     const uint32_t n = std::min(kChunk, nA - r0);
-    CK(cudaMemsetAsync(dBits, 0, (size_t)n * kCapWords * sizeof(uint32_t), st));
+    CK(cudaMemsetAsync(dBits, 0, (size_t)n * kMapWords * sizeof(uint32_t), st));
     k_cap_bake<<<gridFor(h, 8), 256, 0, st>>>(S.alphaRecs + r0, n, dBits, dShadowOk);
     h->kernelLaunches++;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(bits.data(), dBits, (size_t)n * kCapWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(bits.data(), dBits, (size_t)n * kMapWords * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(shadowOk.data() + r0, dShadowOk, n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     for(uint32_t r = 0; r < n; r++)
     {
-      const uint32_t* m = &bits[(size_t)r * kCapWords];
-      uint32_t        caps = 0;
-      for(uint32_t w = 0; w < kCapWords; w++)
-        caps += (uint32_t)__builtin_popcount(m[w]);
-      if(caps == 0)
-        continue;
-      any = true;
-      if(caps == kCapMicro)
-        refOfRec[r0 + r] = kCapAll;
-      else
-      {
-        refOfRec[r0 + r] = (uint32_t)packed.size();
-        packed.insert(packed.end(), m, m + kCapWords);
-      }
+      const uint32_t* m = &bits[(size_t)r * kMapWords];
+      refOfRec[r0 + r] = refOf(m, true);
+      refOfRecS[r0 + r] = shadowOk[r0 + r] ? refOfRec[r0 + r] : refOf(m, false);
     }
   }
   if(!any)
@@ -3631,8 +3699,7 @@ int bakeAlphaCaps(b200pt* h)
     if(recOfSlot[k] != 0xFFFFFFFFu)
       refC[k] = refOfRec[recOfSlot[k]];
   for(uint32_t r = 0; r < nA; r++)
-    if(shadowOk[r])
-      refS[base + r] = refOfRec[r];
+    refS[base + r] = refOfRecS[r];
   DeviceArena     caps;
   const uint32_t* dRefC = caps.upload(refC.data(), refC.size(), st);
   const uint32_t* dRefS = caps.upload(refS.data(), refS.size(), st);
@@ -5283,6 +5350,17 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
       const double* m = &ms[(size_t)b * kStageCount];
       fprintf(stderr, "iter %2d  %8u rays  k_trace %.3f  k_alpha %.3f  k_shade %.3f | %8u shadow rays  k_shadow %.3f | %8u paths  k_resolve %.3f | other %.3f ms\n", b,
                 *hc.trace(b), m[kStageTrace], m[kStageAnyHit], m[kStageShade], *hc.shadow(b), m[kStageShadow], *hc.post(b), m[kStageResolve], m[kStageOther]);
+      // any-hit rounds: paths entering k_alpha in round r and paths sent on to continuation round r
+      for(int kind = 0; kind < 2; kind++)
+      {
+        fprintf(stderr, "         %s any-hit", kind ? "shadow " : "closest");
+        for(int r = 0; r <= h->contRounds; r++)
+          fprintf(stderr, " %u%s", *hc.anyHit(kind, r, b), r < h->contRounds ? "" : "\n");
+        fprintf(stderr, "         %s cont   ", kind ? "shadow " : "closest");
+        for(int r = 0; r < h->contRounds; r++)
+          fprintf(stderr, " %u", *hc.cont(kind, r, b));
+        fprintf(stderr, "\n");
+      }
     }
     fprintf(stderr, "outside the bounce loop: other %.3f ms\n", ms[(size_t)it * kStageCount + kStageOther]);
   }

@@ -1,12 +1,13 @@
 // host_caps_check.cpp — the alpha-cap bake (../alpha_caps.cuh: capBakeCell, the code k_cap_bake runs per cell) compiled for the host
 // through host_shim.h, on records written by tests/test_alpha_caps.py.
-//   host_caps_check in.bin out.bin
+//   host_caps_check in.bin out.bin [holes]
 //   in:  u32 n, then n records: f32 uv[6], i32 w, h, wrapS, wrapT, f32 factor, cutoff, u32 modeFlags, colA, hasTexture,
 //        then (hasTexture) w * h alpha bytes, row-major
-//   out: n x kCapWords u32, the cap bits of every record (bit i = micro-triangle i in ommBary2Index order)
+//   out: n x kCapWords u32, the cap bits of every record (bit i = micro-triangle i in ommBary2Index order); with `holes` its hole bits
 #include "host_shim.h"
 
 #include <cstdio>
+#include <cstring>
 #include <vector>
 
 #include "../alpha_caps.cuh"
@@ -30,6 +31,7 @@ int main(int argc, char** argv)
 {
   if(argc < 3)
     return 2;
+  const bool holes = argc > 3 && std::strcmp(argv[3], "holes") == 0;
   FILE* f = std::fopen(argv[1], "rb");
   FILE* o = std::fopen(argv[2], "wb");
   if(!f || !o)
@@ -54,7 +56,8 @@ int main(int argc, char** argv)
     for(uint32_t k = 0; k < 2 * kCapMicro; k++)
     {
       uint32_t idx;
-      if(capBakeCell(k, uv, w, h, wrapBits, fc[0], fc[1], flags[0], flags[1], flags[2] != 0, alpha8, wrapHost, idx))
+      bool     cap, hole;
+      if(capBakeCell(k, uv, w, h, wrapBits, fc[0], fc[1], flags[0], flags[1], flags[2] != 0, alpha8, wrapHost, idx, cap, hole) && (holes ? hole : cap))
         bits[idx >> 5] |= 1u << (idx & 31u);
     }
     std::fwrite(bits.data(), 4, bits.size(), o);

@@ -30,6 +30,9 @@ struct Cand
 };
 // any-hit candidates kept per tree walk (k_alpha uses that many lanes per path)
 constexpr int kCand = 4;
+// CAPS walks tag the slot of a kept candidate whose micro-triangle is a cap or a hole (alpha_caps.cuh); triangle slots stay below
+// kCandCapsSlots in a scene with caps, and the tags never leave the walk kernels
+constexpr uint32_t kCandCap = 0x80000000u, kCandHole = 0x40000000u, kCandSlot = 0x3FFFFFFFu, kCandCapsSlots = kCandHole;
 // a lane postpones its triangle group while fewer than 1 / 2^kPostponeShift of the warp's active lanes have one (see step())
 constexpr int kPostponeShift = 2;
 
@@ -427,15 +430,19 @@ struct TravState
               if(collectN == KC && shrink)
                 bound = fminf(bound, cand[(KC - 1) * cs].t);
               // a cap passes its any-hit test whatever it draws: nothing behind it is drawn for, so nothing behind it is needed
-              // (the (t, id) order is kept: the box test's widening still admits triangles at t itself)
+              // (the (t, id) order is kept: the box test's widening still admits triangles at t itself).  A kept cap or hole is
+              // tagged in its slot's top bits (kCandCap / kCandHole): its any-hit test needs no texel.
               if(CAPS && shrink)
               {
                 const uint32_t ref = __ldg(&capRef[slot]);
                 if(ref != kCapNone)
                 {
                   const bool fl = (flags & TRI_FLIPPED) != 0;
-                  if(capAt(ref, fl ? v : u, fl ? u : v, [&](uint32_t o) { return __ldg(&capBits[o]); }))
+                  const int  st = capState(ref, fl ? v : u, fl ? u : v, [&](uint32_t o) { return __ldg(&capBits[o]); });
+                  if(st == kMicroCap)
                     bound = fminf(bound, t);
+                  if(st != kMicroOther)
+                    cand[pos * cs].slot = slot | (st == kMicroCap ? kCandCap : kCandHole);
                 }
               }
             }
