@@ -675,21 +675,62 @@ __device__ __forceinline__ PbrMaterial planeMaterial(const FrameParams& F)
   return m;
 }
 
-// H100 (SynthSponza 1080p bench): 256-thread CTAs at <= 255 registers run without spills and beat 512 at <= 128
+// k_shade runs two 256-thread CTAs per SM in 128 registers (H100, SynthSponza 1080p bench: 446 -> 473 Mray/s against one
+// CTA at 159 registers; DESIGN.md section 3).  What a pass carries across its sections besides the path state -- the
+// material record and four hit fields -- is kept per thread in dynamic shared memory (ShadeScratch), so it takes no
+// registers and no local memory.  Bytes per CTA: 2 048 (sRGB table) + 59 392 (material records) + 12 288 (hit fields)
+// = 73 728; two CTAs leave 80 KB of the SM's 228 KB for the walk CTAs (10 KB each) of other frames in flight.
 constexpr int kShadeBlock = 256;
 constexpr int kShadeCtasPerSM = 2;  // CTAs per SM of the persistent shade grid
+// a thread's material record, padded to 58 words: the records of a warp's 32 lanes then start in 16 different banks
+// (56 words would put them in 4), and the BSDF functions still take a plain PbrMaterial by reference
+struct ShadeMaterial
+{
+  PbrMaterial m;
+  float       pad[2];
+};
+static_assert(sizeof(ShadeMaterial) == 58 * 4, "material record stride");
+// the HitState fields read after evaluateMaterial, one float3 each, field-major: lane t of a warp reads word t
+enum : int
+{
+  SHADE_HIT_POS = 0,
+  SHADE_HIT_SHADOW_POS = 1,
+  SHADE_HIT_NRM = 2,
+  SHADE_HIT_GEONRM = 3,
+  SHADE_HIT_FIELDS = 4
+};
+struct ShadeScratch
+{
+  float         lutSrgb[512];  // s_lutSrgb: stageSrgbLut fills the front of the dynamic block
+  ShadeMaterial mat[kShadeBlock];
+  float         hit[SHADE_HIT_FIELDS * 3][kShadeBlock];
+};
+constexpr int kShadeSmem = (int)sizeof(ShadeScratch);
+static_assert(kShadeSmem == 73728, "the byte count stated above");
+// k_shade<0> and k_shade<FEAT_LEAN> keep 146 bytes of spill stores at 128 registers.  k_shade<FEAT_ALL>, twice the code,
+// would keep 162 and runs at 153 registers, one CTA per SM: two were not measured on the scenes that need it.
 template <uint32_t FEAT>
-__global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene S, const __grid_constant__ FrameParams F, const uint32_t* __restrict__ q,
-                                                          const uint32_t* __restrict__ cntIn, uint32_t* qPost, uint32_t* cntPost, uint32_t* qShadow, uint32_t* cntShadow,
-                                                          uint32_t* qNext, uint32_t* cntNext, DevStats* stats)
+constexpr int kShadeMinCtas = FEAT == FEAT_ALL ? 1 : 2;
+template <uint32_t FEAT>
+__global__ void __launch_bounds__(kShadeBlock, kShadeMinCtas<FEAT>) k_shade(PathState P, DevScene S, const __grid_constant__ FrameParams F, const uint32_t* __restrict__ q,
+                                                                            const uint32_t* __restrict__ cntIn, uint32_t* qPost, uint32_t* cntPost, uint32_t* qShadow,
+                                                                            uint32_t* cntShadow, uint32_t* qNext, uint32_t* cntNext, DevStats* stats)
 {
   stageSrgbLut(S.lutSrgb);
   const uint32_t count = *cntIn;
   const uint32_t stride = gridDim.x * blockDim.x;
   // One path per thread per pass.  The kernel is ~12 000 straight-line instructions that every warp walks once per
   // path, so it is bound by instruction fetch (ncu: no_instruction is its top stall, 20 % issue utilisation); the
-  // block-uniform loop with a barrier per pass keeps the eight warps of a 256-thread block inside the same stretch of
-  // code so they share the fetched lines.
+  // block-uniform loop with a barrier per pass keeps the warps of a block inside the same stretch of code so they share
+  // the fetched lines, and two CTAs per SM let each fetched line serve 512 paths.
+  ShadeScratch& scratch = *reinterpret_cast<ShadeScratch*>(s_lutSrgb);
+  PbrMaterial&  pbrMat = scratch.mat[threadIdx.x].m;
+  auto          putHit = [&](int field, float3 v) {
+    scratch.hit[3 * field][threadIdx.x] = v.x;
+    scratch.hit[3 * field + 1][threadIdx.x] = v.y;
+    scratch.hit[3 * field + 2][threadIdx.x] = v.z;
+  };
+  auto getHit = [&](int field) { return f3(scratch.hit[3 * field][threadIdx.x], scratch.hit[3 * field + 1][threadIdx.x], scratch.hit[3 * field + 2][threadIdx.x]); };
   // pass state shared by the four sections of a pass (see the pass loop below)
   uint32_t                  i = 0, flags = 0, seed = 0, scatterBounces = 0, sampleIdx = 0, depth = 0, slot = 0;
   float4                    hr, misc;
@@ -698,8 +739,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
   float                     coneWidth = 0.f, lastSamplePdf = 0.f, hitT = 0.f, worldFoot = 0.f;
   uint2                     meta;
   const b200pt_render_node* nodeP = nullptr;
-  HitState                  hit;
-  PbrMaterial               pbrMat;
+  HitState                  hit;  // sections 1 and 2; sections 3 and 4 read its four fields back with getHit
   DirectLight               directLight;
   bool                      nextEventValid = false;
   bool                      onPlane = false;  // the ray met the infinite ground plane in front of the geometry
@@ -811,6 +851,10 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
   };
   // ---- section 2: material evaluation (three trilinear texture lookups), emission, unlit ----
   auto shadeMaterial = [&]() -> bool {
+    putHit(SHADE_HIT_POS, hit.pos);
+    putHit(SHADE_HIT_SHADOW_POS, hit.shadowPos);
+    putHit(SHADE_HIT_NRM, hit.nrm);
+    putHit(SHADE_HIT_GEONRM, hit.geonrm);
     worldFoot = rayConeWorldFootprint(coneWidth, F.pc.pixelAngle, hitT, hit.geonrm, dir);
     int unlit = 0;
     if(onPlane)
@@ -830,7 +874,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
       const int                    materialIndex = max(0, node.materialID);
       const float                  texGrad = footprintTexGrad(worldFoot, hit.texelDensity, F.pc.texGradScale);
       const b200pt_shade_material& gmat = S.mats[materialIndex];
-      pbrMat = evaluateMaterial<FEAT>(S, gmat, hit, (flags & PF_INSIDE) != 0, texGrad);
+      evaluateMaterial<FEAT>(pbrMat, S, gmat, hit, (flags & PF_INSIDE) != 0, texGrad);
       unlit = gmat.unlit;
     }
 
@@ -851,7 +895,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     // first-hit capture for the NDC depth output of frame 0 and, on DLSS frames, of every frame (gltf_pathtrace.slang:228-232)
     const bool dlss = isDlssFrame(P, F);
     if(depth == 0 && (isFirstFrame(F, i) || dlss))
-      P.firstHit[i] = f4(hit.pos, 1.0f);
+      P.firstHit[i] = f4(getHit(SHADE_HIT_POS), 1.0f);
     // denoiser guides of the first hit (gltf_pathtrace.slang:240-263): base colour and shading normal / roughness, stored as
     // float16_t by the reference.  (maxRoughness is still 0 at depth 0, so the clamp above left pbrMat.roughness as evaluateMaterial
     // returned it.)
@@ -864,11 +908,11 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     if(depth == 0 && dlss)
     {
       // instance motion: the same surface point under the previous frame's objectToWorld (:235-241); the plane does not move
-      float3 prev = hit.pos;
+      float3 prev = getHit(SHADE_HIT_POS);
       if(!onPlane && F.prevObjectToWorld)
       {
         const uint32_t rnode = meta.x & 0x0fffffffu;
-        const float4   objPos = mul_vM(f4(hit.pos, 1.0f), *reinterpret_cast<const Mat4*>(nodeP->worldToObject));
+        const float4   objPos = mul_vM(f4(prev, 1.0f), *reinterpret_cast<const Mat4*>(nodeP->worldToObject));
         prev = xyz(mul_vM(f4(xyz(objPos), 1.0f), *reinterpret_cast<const Mat4*>(F.prevObjectToWorld + 16u * rnode)));
       }
       P.prevHit[i] = f4(prev, 1.0f);
@@ -971,25 +1015,25 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     coneWidth = worldFoot;
 
     // ---- next-event estimation: one light-or-environment sample, MIS (:316-351) ----
-    directLight = sampleLights<FEAT>(S, F, hit.pos, seed);
+    directLight = sampleLights<FEAT>(S, F, getHit(SHADE_HIT_POS), seed);
     if(catcher)
     {
       // handleShadowCatcher, first half (:511-523): the light sample and its shadow ray -- from the plane point itself, unbounded.
       // The shadow factor comes back through the shadow / any-hit kernels in shC; finishPost continues with the second half.
       flags |= PF_CATCHER;
-      if(dot(directLight.direction, hit.nrm) > 0.0f && directLight.pdf != 0.0f)
+      if(dot(directLight.direction, getHit(SHADE_HIT_NRM)) > 0.0f && directLight.pdf != 0.0f)
       {
-        P.shO[i] = f4(hit.pos, kInfinite);
+        P.shO[i] = f4(getHit(SHADE_HIT_POS), kInfinite);
         P.shD[i] = f4(directLight.direction, 0.0f);
         P.shC[i] = f4(1.0f, 1.0f, 1.0f, 0.0f);
         flags |= PF_SHADOW_VALID;
       }
-      P.rayO[i] = f4(hit.pos, coneWidth);  // the incoming direction stays in rayD: the second half looks the environment up along it
+      P.rayO[i] = f4(getHit(SHADE_HIT_POS), coneWidth);  // the incoming direction stays in rayD: the second half looks the environment up along it
       P.misc[i] = f4(misc.x, misc.y, __uint_as_float(flags), __uint_as_float(seed));
       handOff();
       return false;
     }
-    nextEventValid = (dot(directLight.direction, hit.nrm) > 0.0f || pbrMat.diffuseTransmissionFactor > 0.0f) && directLight.pdf != 0.0f;
+    nextEventValid = (dot(directLight.direction, getHit(SHADE_HIT_NRM)) > 0.0f || pbrMat.diffuseTransmissionFactor > 0.0f) && directLight.pdf != 0.0f;
     return true;
   };
   // ---- section 4: BSDF evaluation for the light sample, BSDF sampling, next ray + shadow ray ----
@@ -998,7 +1042,7 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
 #ifdef B200PT_DEBUG
     if(dbgPixel)
       printf("DBG shade pos=%.9g %.9g %.9g nrm=%.9g %.9g %.9g gn=%.9g %.9g %.9g N=%.9g %.9g %.9g rough=%.9g %.9g metal=%.9g base=%.9g %.9g %.9g L=%.9g %.9g %.9g lpdf=%.9g valid=%d seed=%u\n",
-             hit.pos.x, hit.pos.y, hit.pos.z, hit.nrm.x, hit.nrm.y, hit.nrm.z, hit.geonrm.x, hit.geonrm.y, hit.geonrm.z, pbrMat.N.x, pbrMat.N.y, pbrMat.N.z, pbrMat.roughness.x,
+             getHit(SHADE_HIT_POS).x, getHit(SHADE_HIT_POS).y, getHit(SHADE_HIT_POS).z, getHit(SHADE_HIT_NRM).x, getHit(SHADE_HIT_NRM).y, getHit(SHADE_HIT_NRM).z, getHit(SHADE_HIT_GEONRM).x, getHit(SHADE_HIT_GEONRM).y, getHit(SHADE_HIT_GEONRM).z, pbrMat.N.x, pbrMat.N.y, pbrMat.N.z, pbrMat.roughness.x,
              pbrMat.roughness.y, pbrMat.metallic, pbrMat.baseColor.x, pbrMat.baseColor.y, pbrMat.baseColor.z, directLight.direction.x, directLight.direction.y,
              directLight.direction.z, directLight.pdf, (int)nextEventValid, seed);
 #endif
@@ -1032,8 +1076,9 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
         flags |= PF_SPEC_CAPTURE;
       if(sd.event_type != BSDF_EVENT_ABSORB)
       {
-        const float3 offsetDir = dot(dir, hit.geonrm) > 0 ? hit.geonrm : -hit.geonrm;
-        org = safeOffsetRay(hit.pos, offsetDir);
+        const float3 geonrm = getHit(SHADE_HIT_GEONRM);
+        const float3 offsetDir = dot(dir, geonrm) > 0 ? geonrm : -geonrm;
+        org = safeOffsetRay(getHit(SHADE_HIT_POS), offsetDir);
         if((FEAT & (FEAT_TRANSMISSION | FEAT_DIFFUSE_TRANSMISSION)) && (sd.event_type & BSDF_EVENT_TRANSMISSION))
         {
           flags ^= PF_INSIDE;
@@ -1048,9 +1093,10 @@ __global__ void __launch_bounds__(kShadeBlock, 1) k_shade(PathState P, DevScene 
     // ---- shadow ray for the delayed NEE visibility test (:418-426) ----
     if(nextEventValid)
     {
-      const bool   forward = dot(directLight.direction, hit.nrm) > 0.0f;
-      const float3 sDir = forward ? hit.geonrm : -hit.geonrm;
-      const float3 sBase = forward ? hit.shadowPos : hit.pos;
+      const bool   forward = dot(directLight.direction, getHit(SHADE_HIT_NRM)) > 0.0f;
+      const float3 geonrm = getHit(SHADE_HIT_GEONRM);
+      const float3 sDir = forward ? geonrm : -geonrm;
+      const float3 sBase = forward ? getHit(SHADE_HIT_SHADOW_POS) : getHit(SHADE_HIT_POS);
       P.shO[i] = f4(safeOffsetRay(sBase, sDir), directLight.distance);
       P.shD[i] = f4(directLight.direction, 0.0f);
       P.shC[i] = f4(contribution, 0.0f);
@@ -1814,7 +1860,8 @@ __global__ void __launch_bounds__(128) k_shade_state(PathState P, DevScene S, co
   const HitState            hit = fetchHitState(S, slot, hr.y, hr.z, dir, meta, nodeP);
   const float               worldFoot = rayConeWorldFootprint(p[9], p[10], hr.x, hit.geonrm, dir);
   const float               texGrad = footprintTexGrad(worldFoot, hit.texelDensity, p[11]);
-  const PbrMaterial         m = evaluateMaterial<FEAT>(S, S.mats[max(0, nodeP->materialID)], hit, p[8] != 0.0f, texGrad);
+  PbrMaterial               m;
+  evaluateMaterial<FEAT>(m, S, S.mats[max(0, nodeP->materialID)], hit, p[8] != 0.0f, texGrad);
   q[0] = hr.x;
   q[1] = (float)(meta.x & 0x0fffffffu);
   q[2] = (float)nodeP->renderPrimID;
@@ -2757,6 +2804,13 @@ int b200pt_create(b200pt_t** out, int cuda_device)
   cudaDeviceProp prop{};
   need(cudaGetDeviceProperties(&prop, cuda_device));
   h->numSMs = prop.multiProcessorCount > 0 ? prop.multiProcessorCount : 132;
+  // k_shade's ShadeScratch is over the 48 KB of dynamic shared memory a kernel gets unasked, and two of them need the
+  // largest shared-memory carve-out
+  for(const void* shade : {(const void*)k_shade<0u>, (const void*)k_shade<FEAT_LEAN>, (const void*)k_shade<FEAT_ALL>})
+  {
+    need(cudaFuncSetAttribute(shade, cudaFuncAttributeMaxDynamicSharedMemorySize, kShadeSmem));
+    need(cudaFuncSetAttribute(shade, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  }
   h->dStats = h->mem.alloc<DevStats>(1);
   if(h->dStats)
     need(cudaMemset(h->dStats, 0, sizeof(DevStats)));
@@ -5286,7 +5340,7 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
           qShade = L.dQ[4];
         }
         ctx(kStageShade, [&](cudaStream_t st) {
-          shade<<<gS, kShadeBlock, 2048, st>>>(L.P, h->S, F, qShade, C.trace(it), L.dQ[2], C.post(it), L.dQ[3], C.shadow(it), qN, C.trace(it + 1), h->dStats);
+          shade<<<gS, kShadeBlock, kShadeSmem, st>>>(L.P, h->S, F, qShade, C.trace(it), L.dQ[2], C.post(it), L.dQ[3], C.shadow(it), qN, C.trace(it + 1), h->dStats);
         });
         launchWalk(ctx, 1, L.P, L.dQ[3], L.dQ[4], L.dQ[5], C, it, 0);
         ctx(kStageResolve, [&](cudaStream_t st) { k_resolve<<<gridFor(h, 4), 256, 0, st>>>(L.P, h->S, F, L.dQ[2], C.post(it), qN, C.trace(it + 1), h->dStats); });

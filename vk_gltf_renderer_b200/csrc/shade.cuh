@@ -165,7 +165,7 @@ PT_D float footprintTexGrad(float worldFoot, float texelDensity, float texGradSc
 // ---- textures -----------------------------------------------------------------------------------
 // 8-bit sRGB EOTF decode table (same fp32 values as the oracle's), staged in shared memory by every kernel
 // that can touch a texture (divergent indices: constant memory would serialise them)
-extern __shared__ float s_lutSrgb[];
+extern __shared__ __align__(16) float s_lutSrgb[];
 PT_D void stageSrgbLut(const float* __restrict__ lutGlobal)
 {
   for(int i = threadIdx.x; i < 512; i += blockDim.x)
@@ -288,10 +288,11 @@ PT_D float3 multiToSingleScatterAlbedo(float3 rho)
   return f3(1.0f) - t * t;
 }
 
+// writes every field of pbrMat (k_shade passes its record in shared memory: the fields then leave the registers as they
+// are computed, not all at once behind the last texture fetch)
 template <uint32_t FEAT>
-PT_D PbrMaterial evaluateMaterial(const DevScene& S, const b200pt_shade_material& material, const HitState& hit, bool isInside, float texGrad)
+PT_D void evaluateMaterial(PbrMaterial& pbrMat, const DevScene& S, const b200pt_shade_material& material, const HitState& hit, bool isInside, float texGrad)
 {
-  PbrMaterial pbrMat;
 #define PT_TEX(slot) getTexture(S, material.slot, hit.uv0, hit.uv1, texGrad)
   if((FEAT & FEAT_SPECGLOSS) && material.pbrModel == 1)
   {
@@ -470,7 +471,6 @@ PT_D PbrMaterial evaluateMaterial(const DevScene& S, const b200pt_shade_material
   // use it are rejected by b200pt_set_scene, so the factor is always 0 here
   pbrMat.retroreflection = 0.0f;
 #undef PT_TEX
-  return pbrMat;
 }
 
 // ---- alpha + shadow transmission ----------------------------------------------------------------
