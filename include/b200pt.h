@@ -611,6 +611,36 @@ int b200pt_render_views(b200pt_t* h, const b200pt_frame_info* fis, uint32_t n, c
 int b200pt_read_views(b200pt_t* h, uint32_t view, float* host_rgba32f, uint32_t* host_object_ids, float* host_ndc_depth, size_t num_pixels);
 int b200pt_get_views_device(b200pt_t* h, uint32_t view, float** dev_rgba32f, uint32_t** dev_object_ids, float** dev_ndc_depth);
 
+/* Convergence: stop each pixel of an accumulation once its estimated relative error is small enough, so that later frames trace only
+ * the pixels still noisy (the library's own capability; the reference traces every pixel of every frame).  For a pixel p and every
+ * frame f in which p is active (F = frames since the accumulation's first frame, N = samples after the frame, the same for every
+ * active pixel):
+ *   c_f = (r + g + b) / 3 of the frame's clamped sample mean, n_f = numSamples, m = the same luminance of the accumulated RGB after the
+ *   frame, m_prev before it;  M2 += n_f (c_f - m_prev)(c_f - m);  e = sqrt(M2 / ((F - 1) N)) / max(m, floor), +inf while F < 2.
+ * After a frame whose F is a multiple of `interval` (a checkpoint), an active pixel with F >= minFrames and e <= threshold stops: its
+ * image, M2 and stop frame F stay as they are for the rest of the accumulation, and later frames start no path for it.  A stopped
+ * pixel's image is bit-identical to the image of the same accumulation rendered without convergence after frame F - 1; the images do
+ * not depend on frames in flight or frame batching (a batch ends at a checkpoint).  Per pixel of the tile 8 bytes of state.
+ *
+ * b200pt_set_convergence: NULL or threshold 0 turns it off; a negative or NaN threshold or floor, minFrames < 2 or interval < 1 give
+ *   B200PT_E_INVALID.  With floor 0, a pixel whose mean luminance is 0 has e = NaN and never stops: use floor > 0 to let black
+ *   pixels stop.  A frame that fails drops the running accumulation's statistics (the next frame must carry B200PT_PT_FIRST_FRAME).  The settings take effect at the next frame carrying B200PT_PT_FIRST_FRAME, which restarts the statistics;
+ *   frames before it render under the old ones.  While it is on, the frame after a b200pt_resize (or a call that rebuilds the path
+ *   pool) must carry B200PT_PT_FIRST_FRAME (else B200PT_E_INVALID), and more than one view, DLSS frames and
+ *   B200PT_PT_USE_OPTIX_DENOISER frames are refused with B200PT_E_UNSUPPORTED.  Row tiles and interleaved bands keep one mask per tile.
+ * b200pt_read_convergence: synchronises; per pixel of the tile the frame count at which it stopped (0 = active) and e (a stopped
+ *   pixel's at its stop frame), and the number of active pixels.  Any pointer may be NULL.  B200PT_E_INVALID when the current
+ *   accumulation runs without convergence. */
+typedef struct b200pt_convergence
+{
+  float    threshold; /* relative error at which a pixel stops; 0 = off */
+  float    floor;     /* luminance below which the error is taken relative to floor */
+  uint32_t minFrames; /* >= 2: no pixel stops before this many frames */
+  uint32_t interval;  /* >= 1: pixels stop only after frames whose count is a multiple of interval */
+} b200pt_convergence;
+int b200pt_set_convergence(b200pt_t* h, const b200pt_convergence* c);
+int b200pt_read_convergence(b200pt_t* h, uint32_t* host_stop_frame, float* host_rel_error, size_t num_pixels, uint32_t* active_pixels);
+
 /* Let the caller own the accumulation storage (e.g. a torch tensor that NCCL all-gathers):
  * dev_rgba32f must hold tile_rows*width*4 floats on the handle's device. NULL restores the
  * internal buffer. */

@@ -23,6 +23,7 @@ EXPORTS = [
     "b200pt_set_dlss_guides", "b200pt_read_dlss_guides", "b200pt_get_dlss_guides_device",
     "b200pt_update_materials", "b200pt_update_node_materials", "b200pt_update_lights", "b200pt_set_node_visibility",
     "b200pt_set_views", "b200pt_render_views", "b200pt_read_views", "b200pt_get_views_device",
+    "b200pt_set_convergence", "b200pt_read_convergence",
 ]
 
 
@@ -107,6 +108,8 @@ def lib(count_traversal=False):
     L.b200pt_render_views.argtypes = [vp, C.POINTER(abi.FrameInfo), u32, C.POINTER(abi.PushConstant)]
     L.b200pt_read_views.argtypes = [vp, u32, vp, vp, vp, C.c_size_t]
     L.b200pt_get_views_device.argtypes = [vp, u32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
+    L.b200pt_set_convergence.argtypes = [vp, C.POINTER(abi.Convergence)]
+    L.b200pt_read_convergence.argtypes = [vp, vp, vp, C.c_size_t, C.POINTER(u32)]
     for name in EXPORTS:
         getattr(L, name)  # raises AttributeError if a declared symbol is not exported
     _libs[path] = L

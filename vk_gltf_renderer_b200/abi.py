@@ -140,6 +140,11 @@ class DlssGuides(C.Structure):
                 ("depth", C.c_void_p), ("depth_bytes", C.c_size_t), ("spec_hit_dist", C.c_void_p), ("spec_hit_dist_bytes", C.c_size_t)]
 
 
+class Convergence(C.Structure):
+    """b200pt_convergence: per-pixel stopping rule of an accumulation (include/b200pt.h); threshold 0 = off"""
+    _fields_ = [("threshold", C.c_float), ("floor", C.c_float), ("minFrames", C.c_uint32), ("interval", C.c_uint32)]
+
+
 class RenderNodeMapping(C.Structure):
     """b200pt_render_node_mapping == RenderNodeGpuMapping (shaders/world_matrix_io.h.slang:41-47)"""
     _fields_ = [("nodeID", C.c_int32), ("pad0", C.c_int32), ("materialID", C.c_int32), ("renderPrimID", C.c_int32)]

@@ -39,6 +39,7 @@
 
 #include "bvh.h"
 #include "animate.cuh"
+#include "converge.cuh"
 #include "dlss_guides.cuh"
 #include "lbvh.cuh"
 #include "shade.cuh"
@@ -121,6 +122,16 @@ __device__ __forceinline__ void statAdd(unsigned long long* p, unsigned long lon
     atomicAdd(p, v * (unsigned long long)__popc(mask));
 }
 
+// what k_accumulate<true> reads and updates (converge.cuh): per tile pixel M2 and the frame count at which the pixel stopped
+// (0 while active), the accumulation's rule and the frames of the accumulation before this launch's first
+struct ConvergeState
+{
+  float*       m2;
+  uint32_t*    stopFrame;
+  ConvergeRule rule;
+  uint32_t     frames;
+};
+
 // -------------------------------------------------------------------------------------------------
 // camera ray + sample start (samplePixel head: gltf_pathtrace.slang:502-530; getRay: pathtrace_functions.h.slang:791-811)
 // -------------------------------------------------------------------------------------------------
@@ -201,12 +212,18 @@ __device__ void finalizeSample(const PathState& P, const FrameParams& F, uint32_
 // -------------------------------------------------------------------------------------------------
 // kernels
 // -------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_constant__ FrameParams F, uint32_t* qTrace, uint32_t* cnt0, DevStats* stats)
+// MASKED (convergence on, after the accumulation's first frame): slots of pixels that stopped (stopFrame != 0) start no path and
+// the others are queued; otherwise every slot starts one and the queue is the identity
+template <bool MASKED>
+__global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_constant__ FrameParams F, uint32_t* qTrace, uint32_t* cnt0, DevStats* stats,
+                                                const uint32_t* __restrict__ stopFrame)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
   for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.numPaths; i += stride)
   {
     const uint32_t px = pixelOf(F, i);
+    if(MASKED && stopFrame[px] != 0u)
+      continue;
     const uint32_t x = px % (uint32_t)F.width;
     const uint32_t y = pixelRow(F, px);
     uint32_t       seed = xxhash32(x, y, (uint32_t)F.pc.frameCount + frameOf(F, i));
@@ -230,9 +247,15 @@ __global__ void __launch_bounds__(256) k_raygen(PathState P, const __grid_consta
       P.dlssSpec[i] = make_uint2(0u, 0u);            // specularAlbedo 0, specularHitDist 0
     }
     startSample(P, F, i, seed, jitter, 0u);
-    qTrace[i] = i;
+    if(MASKED)
+    {
+      queuePush(qTrace, cnt0, i);
+      statAdd(&stats->pathsStarted, 1ull);
+    }
+    else
+      qTrace[i] = i;
   }
-  if(blockIdx.x == 0 && threadIdx.x == 0)
+  if(!MASKED && blockIdx.x == 0 && threadIdx.x == 0)
   {
     *cnt0 = F.numPaths;
     atomicAdd(&stats->pathsStarted, (unsigned long long)F.numPaths);
@@ -1400,12 +1423,20 @@ __global__ void __launch_bounds__(256) k_resolve(PathState P, DevScene S, const 
 // first frame also the NDC depth of the last sample's first hit (:600-616; Vulkan [0,1] range, 1 = far / miss).  A DLSS frame
 // replaces the image like a first frame (:619-622).  With views, slot block v updates view v's image: view 0 is `accum` / `ndcDepth`,
 // view v > 0 starts at viewAccum / viewDepth + (v - 1) * pixels.
+// MASKED (convergence on, one view): pixels that stopped are left untouched; the others also update M2 and, after a checkpoint
+// frame, may stop (converge.cuh).  The first frame of an accumulation restarts every pixel's statistics.
+template <bool MASKED>
 __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_constant__ FrameParams F, float4* __restrict__ accum, float* __restrict__ ndcDepth,
-                                                    float4* __restrict__ viewAccum, float* __restrict__ viewDepth)
+                                                    float4* __restrict__ viewAccum, float* __restrict__ viewDepth, ConvergeState cv)
 {
   const uint32_t stride = gridDim.x * blockDim.x;
   for(uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < F.pixels * (uint32_t)F.views; i += stride)
   {
+    const bool first = (F.pc.flags & B200PT_PT_FIRST_FRAME) != 0;
+    if(MASKED && !first && cv.stopFrame[i] != 0u)
+      continue;
+    float    m2 = MASKED && !first ? cv.m2[i] : 0.0f;
+    uint32_t stop = 0u;
     float4* const out = i < F.pixels ? accum + i : viewAccum + (i - F.pixels);
     float4        img = f4(0.f, 0.f, 0.f, 0.f);
     // the frames of a batch are folded in frame order, each with the sample counts its own push constants would have carried
@@ -1437,9 +1468,24 @@ __global__ void __launch_bounds__(256) k_accumulate(PathState P, const __grid_co
         const float  after = (float)(totalSamples + F.pc.numSamples);
         const float4 old = img;
         img = f4((old.x * total + c.x * n) / after, (old.y * total + c.y * n) / after, (old.z * total + c.z * n) / after, (old.w * total + c.w * n) / after);
+        if(MASKED)
+          m2 = convergeUpdate(m2, n, convergeLum(c), convergeLum(old), convergeLum(img));
+      }
+      if(MASKED)
+      {
+        const uint32_t frames = cv.frames + (uint32_t)b + 1u;
+        if(convergeStops(cv.rule, m2, frames, (float)(F.pc.totalSamples + (b + 1) * F.pc.numSamples), convergeLum(img)))
+          stop = frames;
       }
     }
     *out = img;
+    if(MASKED)
+    {
+      cv.m2[i] = m2;
+      // (only a first frame's restart or a stop changes the word; the next frame's k_raygen may already read it)
+      if(first || stop != 0u)
+        cv.stopFrame[i] = stop;
+    }
   }
 }
 
@@ -2246,6 +2292,24 @@ struct b200pt
   float4*               dViewAccum = nullptr;
   uint32_t*             dViewSelect = nullptr;
   float*                dViewDepth = nullptr;
+  // convergence (b200pt_set_convergence): `next` is latched into `cur` by the next frame carrying B200PT_PT_FIRST_FRAME (threshold 0:
+  // off).  While `cur` is on, frames after the first skip the pixels that stopped; the frames' lanes wait on `maskReady`, recorded
+  // after each accumulate that can change the stop mask (the first frame's and a checkpoint's), so the images do not depend on
+  // frames in flight or batching.  The per-pixel state (M2, stop frame) lives in convMem, allocated at the first latch after a resize.
+  struct Convergence
+  {
+    b200pt_convergence next{};
+    b200pt_convergence cur{};
+    bool               latched = false;   // `cur` runs the current accumulation (its first frame was submitted since the pool was built)
+    uint32_t           submitted = 0;     // frames of the accumulation handed to b200pt_render_frame
+    uint32_t           launched = 0;      // ... of which launched
+    std::vector<float> samplesAfter;      // N after frame F, at [F - 1]
+    DeviceArena        mem;
+    float*             dM2 = nullptr;
+    uint32_t*          dStop = nullptr;
+    cudaEvent_t        maskReady = nullptr;
+  };
+  Convergence        conv;
   int                numLanes = 4;   // frames in flight (b200pt_set_frames_in_flight)
   uint64_t           frameSerial = 0;
   int                lastLane = -1;
@@ -2502,6 +2566,10 @@ void freePool(b200pt* h)
   h->dViewSelect = nullptr;
   h->dViewDepth = nullptr;
   h->numPaths = 0;
+  h->conv.latched = false;  // the images are cleared: an accumulation with convergence on needs a first frame again
+  h->conv.mem.release();
+  h->conv.dM2 = nullptr;
+  h->conv.dStop = nullptr;
   for(int l = 0; l < b200pt::kMaxLanes; l++)
   {
     h->lanes[l].P = PathState{};
@@ -2827,6 +2895,7 @@ int b200pt_create(b200pt_t** out, int cuda_device)
       need(growEventPool(h, 16384));
     }
   }
+  need(cudaEventCreateWithFlags(&h->conv.maskReady, cudaEventDisableTiming));
   for(int l = 0; l < b200pt::kMaxLanes; l++)
   {
     b200pt::Lane& L = h->lanes[l];
@@ -2896,6 +2965,8 @@ void b200pt_destroy(b200pt_t* h)
   }
   if(h->tlBase)
     cudaEventDestroy(h->tlBase);
+  if(h->conv.maskReady)
+    cudaEventDestroy(h->conv.maskReady);
   if(h->timeline)
     fclose(h->timeline);
   cudaStreamDestroy(h->stream);
@@ -5098,11 +5169,65 @@ static int checkFrame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_pus
   return B200PT_OK;
 }
 
+// the convergence side of a frame about to be submitted: the refusals, the latch of the settings at a first frame (after the previous
+// accumulation's pending frames are launched under its own) and the frame count of the running accumulation
+static int convergeFrame(b200pt_t* h, const b200pt_push_constant* pc, const char* who)
+{
+  b200pt::Convergence& c = h->conv;
+  const bool           first = (pc->flags & B200PT_PT_FIRST_FRAME) != 0;
+  const std::string    name(who);
+  if(!first && c.cur.threshold > 0.0f && !c.latched)
+  {
+    h->err = name + ": with convergence on, the images were cleared (resize or pool rebuild): the next frame must carry B200PT_PT_FIRST_FRAME";
+    return B200PT_E_INVALID;
+  }
+  const bool on = first ? c.next.threshold > 0.0f : c.latched;
+  if(on && (pc->flags & (B200PT_PT_USE_DLSS | B200PT_PT_USE_OPTIX_DENOISER)))
+  {
+    h->err = name + ": convergence stops pixels of the accumulation; the DLSS and OptiX-denoiser frames need every pixel (b200pt_set_convergence(h, NULL))";
+    return B200PT_E_UNSUPPORTED;
+  }
+  if(on && h->views > 1)
+  {
+    h->err = name + ": convergence works on one view (b200pt_set_views(h, 1))";
+    return B200PT_E_UNSUPPORTED;
+  }
+  if(first)
+  {
+    if(const int rc = flushPending(h))
+      return rc;
+    if(on && !c.dM2)
+    {
+      DeviceArena A;
+      float* const    m2 = A.alloc<float>(h->numPaths);
+      uint32_t* const stop = A.alloc<uint32_t>(h->numPaths);
+      if(!A.ok())
+        return failed(h, A, "convergence state");
+      c.mem = std::move(A);
+      c.dM2 = m2;
+      c.dStop = stop;
+    }
+    c.cur = c.next;
+    c.latched = on;
+    c.submitted = 0;
+    c.launched = 0;
+    c.samplesAfter.clear();
+  }
+  if(c.latched)
+  {
+    c.submitted++;
+    c.samplesAfter.push_back((float)(pc->totalSamples + pc->numSamples));
+  }
+  return B200PT_OK;
+}
+
 int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc)
 {
   if(!h || !fi || !pc)
     return B200PT_E_INVALID;
   if(const int rc = checkFrame(h, fi, pc, "b200pt_render_frame"))
+    return rc;
+  if(const int rc = convergeFrame(h, pc, "b200pt_render_frame"))
     return rc;
   if(h->batch <= 1)
     return launchFrames(h, fi, pc, 1);
@@ -5136,7 +5261,8 @@ int b200pt_render_frame(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
     h->pendingPc = *pc;
   }
   h->pendingCount++;
-  if(h->pendingCount >= h->batch)
+  // with convergence on, a batch ends at a checkpoint: the frames after it start from the mask it leaves
+  if(h->pendingCount >= h->batch || (h->conv.latched && h->conv.submitted % h->conv.cur.interval == 0u))
     return flushPending(h);
   return B200PT_OK;
 }
@@ -5150,6 +5276,11 @@ int b200pt_set_views(b200pt_t* h, int n)
   if(n > 1 && h->batch > 1)
   {
     h->err = "b200pt_set_views: more than one view needs frame batching off (b200pt_set_frame_batch(h, 1))";
+    return B200PT_E_UNSUPPORTED;
+  }
+  if(n > 1 && (h->conv.next.threshold > 0.0f || h->conv.latched))
+  {
+    h->err = "b200pt_set_views: more than one view needs convergence off (b200pt_set_convergence(h, NULL))";
     return B200PT_E_UNSUPPORTED;
   }
   if(const int rc = enter(h, false))
@@ -5191,6 +5322,8 @@ int b200pt_render_views(b200pt_t* h, const b200pt_frame_info* fis, uint32_t n, c
     return B200PT_E_UNSUPPORTED;
   }
   if(const int rc = checkFrame(h, &fis[0], pc, "b200pt_render_views"))
+    return rc;
+  if(const int rc = convergeFrame(h, pc, "b200pt_render_views"))
     return rc;
   if(const int rc = flushPending(h))
     return rc;
@@ -5244,6 +5377,74 @@ int b200pt_get_views_device(b200pt_t* h, uint32_t view, float** dev_rgba32f, uin
   return B200PT_OK;
 }
 
+int b200pt_set_convergence(b200pt_t* h, const b200pt_convergence* c)
+{
+  if(!h)
+    return B200PT_E_INVALID;
+  b200pt_convergence v{};  // off
+  if(c && c->threshold != 0.0f)
+  {
+    if(!(c->threshold > 0.0f) || !(c->floor >= 0.0f) || c->minFrames < 2u || c->interval < 1u)
+    {
+      h->err = "b200pt_set_convergence: threshold and floor must be >= 0 (not NaN), minFrames >= 2 and interval >= 1";
+      return B200PT_E_INVALID;
+    }
+    if(h->views > 1)
+    {
+      h->err = "b200pt_set_convergence: convergence works on one view (b200pt_set_views(h, 1))";
+      return B200PT_E_UNSUPPORTED;
+    }
+    v = *c;
+  }
+  h->conv.next = v;
+  return B200PT_OK;
+}
+
+int b200pt_read_convergence(b200pt_t* h, uint32_t* host_stop_frame, float* host_rel_error, size_t num_pixels, uint32_t* active_pixels)
+{
+  if(!h || h->numPaths == 0 || ((host_stop_frame || host_rel_error) && num_pixels < (size_t)h->numPaths))
+    return B200PT_E_INVALID;
+  if(const int rc = enter(h, false))
+    return rc;
+  const b200pt::Convergence& c = h->conv;
+  if(!c.latched)
+  {
+    h->err = "b200pt_read_convergence: convergence is off in the current accumulation";
+    return B200PT_E_INVALID;
+  }
+  const size_t          n = h->numPaths;
+  std::vector<uint32_t> stop(n);
+  std::vector<float>    m2(host_rel_error ? n : 0);
+  std::vector<float4>   img(host_rel_error ? n : 0);
+  CK(cudaMemcpyAsync(stop.data(), c.dStop, n * 4, cudaMemcpyDeviceToHost, h->stream));
+  if(host_rel_error)
+  {
+    CK(cudaMemcpyAsync(m2.data(), c.dM2, n * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(img.data(), h->dAccum, n * 16, cudaMemcpyDeviceToHost, h->stream));
+  }
+  CK(cudaStreamSynchronize(h->stream));
+  const ConvergeRule rule{c.cur.threshold, c.cur.floor, c.cur.minFrames, c.cur.interval};
+  uint32_t           active = 0;
+  for(size_t i = 0; i < n; i++)
+  {
+    active += stop[i] == 0u;
+    // a stopped pixel's image and M2 are those of its stop frame: its error is the one that stopped it
+    const uint32_t frames = stop[i] ? stop[i] : c.launched;
+    if(frames == 0u || frames > c.samplesAfter.size())
+    {
+      h->err = "b200pt_read_convergence: the frame counts of the accumulation are inconsistent";
+      return B200PT_E_INVALID;
+    }
+    if(host_rel_error)
+      host_rel_error[i] = convergeRelError(rule, m2[i], frames, c.samplesAfter[frames - 1], convergeLum(img[i]));
+  }
+  if(host_stop_frame)
+    memcpy(host_stop_frame, stop.data(), n * 4);
+  if(active_pixels)
+    *active_pixels = active;
+  return B200PT_OK;
+}
+
 static int flushPending(b200pt_t* h)
 {
   if(h->pendingCount == 0)
@@ -5262,7 +5463,22 @@ int b200pt_flush(b200pt_t* h)
 
 // enqueues the launch chain of `count` consecutive frames (count > 1: one batched wavefront, FrameParams::batch), or with viewFis
 // (count 1) of the handle's views, whose poses replace fi's (FrameParams::views)
+static int launchChain(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count, const b200pt_frame_info* viewFis);
+
+// a frame chain that failed leaves the convergence statistics of the running accumulation incomplete: they are dropped, and while
+// convergence is on the next frame must start a new accumulation
 static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count, const b200pt_frame_info* viewFis)
+{
+  const int rc = launchChain(h, fi, pc, count, viewFis);
+  if(rc && h->conv.latched)
+  {
+    h->conv.latched = false;
+    h->err += " (the accumulation's convergence state is lost: the next frame must carry B200PT_PT_FIRST_FRAME)";
+  }
+  return rc;
+}
+
+static int launchChain(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_push_constant* pc, int count, const b200pt_frame_info* viewFis)
 {
   CK(cudaSetDevice(h->device));
   FrameParams F;
@@ -5310,7 +5526,19 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   CK(cudaMemsetAsync(L.dCounters, 0, sizeof(uint32_t) * kCounterArrays * kMaxIters, L.stream));
   Launcher ctx{h, L.stream, laneIdx, h->frameSerial - 1, -1, h->profiling || h->timeline != nullptr, F.numPaths};
   const int gridWide = gridFor(h, 8);
-  ctx(kStageOther, [&](cudaStream_t st) { k_raygen<<<gridWide, 256, 0, st>>>(L.P, F, L.dQ[0], C.trace(0), h->dStats); });
+  // convergence: after the accumulation's first frame, the stop mask as the last checkpoint left it selects the paths to start
+  const bool          converge = h->conv.latched;
+  const bool          masked = converge && !(pc->flags & B200PT_PT_FIRST_FRAME);
+  const ConvergeState cv{h->conv.dM2, h->conv.dStop, {h->conv.cur.threshold, h->conv.cur.floor, h->conv.cur.minFrames, h->conv.cur.interval}, h->conv.launched};
+  if(converge)
+    h->conv.launched += (uint32_t)count;
+  if(masked)
+  {
+    CK(cudaStreamWaitEvent(L.stream, h->conv.maskReady, 0));
+    ctx(kStageOther, [&](cudaStream_t st) { k_raygen<true><<<gridWide, 256, 0, st>>>(L.P, F, L.dQ[0], C.trace(0), h->dStats, cv.stopFrame); });
+  }
+  else
+    ctx(kStageOther, [&](cudaStream_t st) { k_raygen<false><<<gridWide, 256, 0, st>>>(L.P, F, L.dQ[0], C.trace(0), h->dStats, nullptr); });
 
   int it = 0;  // bounces run
   if(pc->maxDepth > 0)
@@ -5368,7 +5596,14 @@ static int launchFrames(b200pt_t* h, const b200pt_frame_info* fi, const b200pt_p
   ctx.lane = -1;
   if(pc->flags & B200PT_PT_FIRST_FRAME)
     ctx(kStageOther, [&](cudaStream_t st) { k_select<<<gridWide, 128, 0, st>>>(h->S, F, h->dSelect, h->dViewSelect, h->dStats); });
-  ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth, h->dViewAccum, h->dViewDepth); });
+  if(converge)
+  {
+    ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<true><<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth, h->dViewAccum, h->dViewDepth, cv); });
+    if(!masked || h->conv.launched % cv.rule.interval == 0u)
+      CK(cudaEventRecord(h->conv.maskReady, h->stream));
+  }
+  else
+    ctx(kStageOther, [&](cudaStream_t st) { k_accumulate<false><<<gridWide, 256, 0, st>>>(L.P, F, h->dAccum, h->dNdcDepth, h->dViewAccum, h->dViewDepth, ConvergeState{}); });
   if((pc->flags & B200PT_PT_USE_OPTIX_DENOISER) && h->dGuide)
     ctx(kStageOther, [&](cudaStream_t st) { k_guide<<<gridWide, 256, 0, st>>>(L.P, F, h->dGuide); });
   if((pc->flags & B200PT_PT_USE_DLSS) && h->dDlss)

@@ -5,7 +5,9 @@
 //   b200pt_headless --headless --size W H --frames N --maxFrames N --ptSamples S --ptAdaptiveSampling 0 --renderSystem 0
 //                   --envSystem 1 --scenefile scene.glb [--hdrfile env.hdr] [extra args]
 // plus  --scene scene.b2sc  (a pre-converted blob), --warmupFrames K, --device G, --framesInFlight L, --out image.pfm,
-// --outRaw image.f32.  A .gltf / .glb scene is converted on the fly by the package's own loader
+// --outRaw image.f32, and the library's own convergence flags (not the reference's): --ptConvergenceThreshold T (0 = off),
+// --ptConvergenceMinFrames M (16) and --ptConvergenceInterval I (8).  With a threshold the run ends at --frames or after the first
+// checkpoint at which no pixel is still active, whichever comes first (include/b200pt.h, b200pt_set_convergence).  A .gltf / .glb scene is converted on the fly by the package's own loader
 // (python -m vk_gltf_renderer_b200.convert).  Flags of the reference application that have no meaning for this backend are
 // skipped with a note on stderr; --renderSystem other than 0 (path tracer) and --envSystem 0 (physical sky) are errors.
 //
@@ -113,6 +115,7 @@ int main(int argc, char** argv)
   std::string scenePath, hdrPath, outPath, rawPath, tmpBlob, tonemappedPath, writeBlobPath;
   int         width = 1920, height = 1080, frames = 16, warmupFrames = 1, framesInFlight = 0;  // warm-up: src/benchmarking.hpp:128
   int         adaptiveSampling = 0, frameBatch = 0;
+  b200pt_convergence convergence{0.0f, 1e-3f, 16u, 8u};
   Resources   res;
   PathTracer  pt;
   try
@@ -181,6 +184,12 @@ int main(int argc, char** argv)
         res.tonemapperData.exposure = std::stof(next());
       else if(a == "--outRaw")
         rawPath = next();
+      else if(a == "--ptConvergenceThreshold")
+        convergence.threshold = std::stof(next());
+      else if(a == "--ptConvergenceMinFrames")
+        convergence.minFrames = (uint32_t)std::stoul(next());
+      else if(a == "--ptConvergenceInterval")
+        convergence.interval = (uint32_t)std::stoul(next());
       else if(a.rfind("--pt", 0) == 0)
       {
         if(!pt.setParameter(a.substr(2), next()))
@@ -243,6 +252,9 @@ int main(int argc, char** argv)
       pt.setFramesInFlight(framesInFlight);
     if(frameBatch > 0)
       pt.setFrameBatch(frameBatch);
+    const bool converge = convergence.threshold != 0.0f;
+    if(converge && b200pt_set_convergence(pt.handle(), &convergence) != B200PT_OK)
+      throw Error(std::string("b200pt_set_convergence: ") + b200pt_last_error(pt.handle()));
 
     // frame loop with the reference's warm-up split (benchmarking.cpp: measured timer starts after warmupFrames)
     using clock = std::chrono::steady_clock;
@@ -259,6 +271,19 @@ int main(int argc, char** argv)
       }
       res.frameCount++;
       pt.onRender(res);
+      if(converge && (f + 1) % (int)convergence.interval == 0)
+      {
+        // the count synchronises, so it is read at checkpoints only: the mask changes nowhere else
+        uint32_t active = 0;
+        if(b200pt_read_convergence(pt.handle(), nullptr, nullptr, 0, &active) != B200PT_OK)
+          throw Error(std::string("b200pt_read_convergence: ") + b200pt_last_error(pt.handle()));
+        if(active == 0)
+        {
+          std::printf("HEADLESS_CONVERGED frame=%d frames=%d: no pixel is active\n", f, f + 1);
+          frames = f + 1;
+          break;
+        }
+      }
       if((f + 1) % 50 == 0 && f + 1 < frames)
       {
         // progress records like updateHeadlessProgressIfNeeded (src/benchmarking.cpp:215-238), every 50 frames; the

@@ -456,6 +456,24 @@ class PathTracer:
         self._ck(self._L.b200pt_get_views_device(self._h, view, C.byref(rgba), C.byref(ids), C.byref(depth)), "b200pt_get_views_device")
         return rgba.value, ids.value, depth.value
 
+    def set_convergence(self, threshold, floor=1e-3, min_frames=16, interval=8):
+        """stop each pixel of the next accumulation once its relative error e <= threshold (include/b200pt.h, DESIGN.md §2
+        "Convergence"); threshold 0 turns it off.  Takes effect at the next frame with frameCount 0."""
+        c = abi.Convergence(threshold, floor, min_frames, interval)
+        self._ck(self._L.b200pt_set_convergence(self._h, C.byref(c)), "b200pt_set_convergence")
+        self._convergence = c if threshold != 0 else None
+
+    def read_convergence(self):
+        """(stop frame uint32 [rows, W] (0 = active), relative error float32 [rows, W], active pixels) of the current accumulation"""
+        w, _ = self._size
+        rows = self._tile[1]
+        stop = np.empty((rows, w), np.uint32)
+        err = np.empty((rows, w), np.float32)
+        active = C.c_uint32()
+        self._ck(self._L.b200pt_read_convergence(self._h, stop.ctypes.data_as(C.c_void_p), err.ctypes.data_as(C.c_void_p), stop.size, C.byref(active)),
+                 "b200pt_read_convergence")
+        return stop, err, active.value
+
     def accum_device_ptr(self):
         p, n = C.c_void_p(), C.c_size_t()
         self._ck(self._L.b200pt_get_accum_device(self._h, C.byref(p), C.byref(n)), "b200pt_get_accum_device")
@@ -509,19 +527,24 @@ class PathTracer:
                  "b200pt_shade_state")
 
 
-def render_headless(resources, frames, *, pt=None, device=0, **pt_params):
+def render_headless(resources, frames, *, pt=None, device=0, until_converged=False, **pt_params):
     """The reference's headless loop (src/main.cpp:133-136 + nvapp frame loop, SURVEY.md §3.1):
-    frameCount runs 0..frames-1, each frame adds ptSamples spp.  Returns (PathTracer, accum RGBA32F)."""
+    frameCount runs 0..frames-1, each frame adds ptSamples spp.  Returns (PathTracer, accum RGBA32F).
+    until_converged: with pt.set_convergence on, the loop also ends after the first checkpoint at which no pixel is active (the
+    count is read at checkpoints only, since the read synchronises); resources.frameCount is then the last frame rendered."""
     own = pt is None
     if own:
         pt = PathTracer(device)
         for k, v in pt_params.items():
             setattr(pt, k, v)
         pt.onAttach(resources)
+    conv = getattr(pt, "_convergence", None) if until_converged else None
     resources.frameCount = -1
     # (the headless run raises maxFrames to the frame count: BenchmarkController::alignMaxFramesForHeadless, so no cap applies)
     for _ in range(frames):
         resources.frameCount += 1
         pt.onRender(None, resources)
+        if conv is not None and (resources.frameCount + 1) % conv.interval == 0 and pt.read_convergence()[2] == 0:
+            break
     img = pt.read_accum()
     return pt, img
