@@ -21,8 +21,8 @@ def checker(tmp_path_factory):
     if not os.path.exists(os.path.join(CUDA_INC, "cuda_runtime.h")):
         pytest.skip("CUDA headers not found")
     exe = str(tmp_path_factory.mktemp("hostcheck") / "host_traverse_check")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-o", exe, os.path.join(CSRC, "tools", "host_traverse_check.cpp"),
-                           os.path.join(CSRC, "bvh.cpp")])
+    subprocess.check_call(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-I" + os.path.join(ROOT, "include"), "-o", exe,
+                           os.path.join(CSRC, "tools", "host_traverse_check.cpp"), os.path.join(CSRC, "bvh.cpp")])
     return exe
 
 

@@ -44,14 +44,8 @@ PT_D uint32_t globalId(const LbvhWork& W, uint32_t local) { return W.subset ? W.
 
 PT_D void lbvhBounds(uint32_t i, const LbvhWork& W)
 {
-  const float* T = W.inRec + (size_t)globalId(W, i) * 12;
-  float        lo[3], hi[3];
-  for(int a = 0; a < 3; a++)
-  {
-    const float v0 = T[a], v1 = T[a] + T[4 + a], v2 = T[a] + T[8 + a];
-    lo[a] = fminf(v0, fminf(v1, v2));
-    hi[a] = fmaxf(v0, fmaxf(v1, v2));
-  }
+  float lo[3], hi[3];
+  triangleBox(W.inRec + (size_t)globalId(W, i) * 12, lo, hi);
   W.primLo[i] = make_float4(lo[0], lo[1], lo[2], 0.f);
   W.primHi[i] = make_float4(hi[0], hi[1], hi[2], 0.f);
   for(int a = 0; a < 3; a++)

@@ -16,6 +16,20 @@
 
 namespace pt {
 
+// box of the triangle the walks intersect (v0, v0 + e1, v0 + e2: T is its 12-float record), padded like the host builder's leaf
+// boxes (bvh.cpp) because the vertex sums are rounded: both builders and the refit bound a triangle the same way
+PT_D void triangleBox(const float* T, float lo[3], float hi[3])
+{
+  for(int a = 0; a < 3; a++)
+  {
+    const float v0 = T[a], v1 = T[a] + T[4 + a], v2 = T[a] + T[8 + a];
+    const float l = fminf(v0, fminf(v1, v2)), h = fmaxf(v0, fmaxf(v1, v2));
+    const float pad = fmaxf(fabsf(l), fabsf(h)) * 4e-7f + 1e-30f;
+    lo[a] = l - pad;
+    hi[a] = h + pad;
+  }
+}
+
 // conservative quantisation of one node, the host builder's arithmetic (bvh.cpp "quantisation frame")
 PT_D void quantiseNode(float* N, const float lo[3], const float hi[3], const float clo[8][3], const float chi[8][3], uint32_t present)
 {
@@ -88,12 +102,12 @@ PT_D void refitNode(uint32_t node, float* nodes, const float* tris, float4* node
       }
       for(uint32_t k = 0; k < count; k++)
       {
-        const float* T = tris + (size_t)(first + k) * 12;
+        float tlo[3], thi[3];
+        triangleBox(tris + (size_t)(first + k) * 12, tlo, thi);
         for(int a = 0; a < 3; a++)
         {
-          const float v0 = T[a], v1 = T[a] + T[4 + a], v2 = T[a] + T[8 + a];
-          clo[s][a] = fminf(clo[s][a], fminf(v0, fminf(v1, v2)));
-          chi[s][a] = fmaxf(chi[s][a], fmaxf(v0, fmaxf(v1, v2)));
+          clo[s][a] = fminf(clo[s][a], tlo[a]);
+          chi[s][a] = fmaxf(chi[s][a], thi[a]);
         }
       }
     }

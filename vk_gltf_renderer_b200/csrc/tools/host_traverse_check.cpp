@@ -1,13 +1,18 @@
 // host_traverse_check.cpp — the device traversal source (traverse.cuh: node decode with the PRMT plane conversion, octant
 // order, compressed stack, postponed groups, single-tree closest / shadow walks with candidate lists, lower bounds, refinement
 // of the opaque hit in continuation walks) compiled for the host through host_shim.h and checked against brute force over all
-// triangles, on the tree the product's builder (bvh.cpp) makes.  A third of the triangles is flagged non-opaque.
+// triangles, on a tree of either builder.  A third of the triangles is flagged non-opaque.
 //
-//   host_traverse_check dump.bin [maxRays] [opaqueMod] [ommLevel]   (dump format of scripts/dump_bvh_input.py: triangles + rays)
+//   host_traverse_check dump.bin [maxRays] [opaqueMod] [ommLevel] [tree] [ownSegment] [hits.bin]
+//   (dump format of scripts/dump_bvh_input.py: triangles + rays)
 //
 // ommLevel > 0: every non-opaque triangle gets an opacity micromap of that subdivision level (4-state format, states from a hash of
 // triangle and micro-triangle index; every 7th triangle a FULLY_TRANSPARENT / FULLY_OPAQUE special state instead) and the walks run
 // with the lookup of omm.cuh: an OPAQUE micro-triangle must behave like an opaque triangle, a TRANSPARENT one like no triangle.
+// tree: 0 the host builder's tree (bvh.cpp), 1 the device builder's tree (lbvh.cuh, run thread after thread), 2 the host builder's
+// tree after every third triangle moved (by 5 % of the scene's extent, squashed along y) and the tree was refitted (refit.cuh).
+// ownSegment: 0 every ray from t = 0, odd rays to their tmax and even rays cut at 3; 1 every ray on its own (tmin, tmax).
+// hits.bin: the brute-force hits of every ray, (ray, gid, t, u, v, det) as 6 x 4 bytes, for the float64 classification of the tests.
 //
 // Checks, per ray, against the sorted brute-force hit list (the triangle test is the same fma chain, so bit for bit):
 // (1) closest protocol of k_trace / k_alpha with every candidate rejected: walks resumed behind the last candidate until a walk
@@ -23,7 +28,7 @@
 #include <cstdlib>
 #include <vector>
 
-#include "../traverse.cuh"
+#include "../lbvh.cuh"
 
 using namespace pt;
 
@@ -48,6 +53,9 @@ int main(int argc, char** argv)
   // deep candidate lists and many continuation walks)
   const int opaqueMod = argc > 3 ? std::atoi(argv[3]) : 3;
   auto isOpaque = [&](uint32_t i) { return opaqueMod > 0 ? (i % (uint32_t)opaqueMod) != 0 : (i % (uint32_t)(-opaqueMod)) == 0; };
+  const int  treeKind = argc > 5 ? std::atoi(argv[5]) : 0;
+  const bool ownSegment = argc > 6 && std::atoi(argv[6]) != 0;
+  FILE*      hitsOut = argc > 7 ? std::fopen(argv[7], "wb") : nullptr;
   std::vector<FlatTri>  tris(nT);
   std::vector<uint32_t> gids(nT);
   for(uint32_t i = 0; i < nT; i++)
@@ -56,7 +64,83 @@ int main(int argc, char** argv)
     tris[i].rnode = 0; tris[i].prim = i; tris[i].flags = TRI_NOCULL | (isOpaque(i) ? TRI_OPAQUE : 0u); gids[i] = i;
   }
   WideBvh B;
-  buildWideBvh(tris, gids, 0, B);
+  if(treeKind == 1)
+  {
+    // the device builder over every triangle, its passes in launch order
+    std::vector<float> rec((size_t)nT * 12);
+    for(uint32_t i = 0; i < nT; i++)
+    {
+      float* R = &rec[(size_t)i * 12];
+      std::memcpy(R, tris[i].v0, 12); std::memcpy(R + 4, tris[i].e1, 12); std::memcpy(R + 8, tris[i].e2, 12);
+      R[3] = __uint_as_float(tris[i].flags << 28); R[7] = __uint_as_float(i); R[11] = __uint_as_float(i);
+    }
+    const uint32_t m = nT;
+    uint32_t       M = 1;
+    while(M < m) M <<= 1;
+    std::vector<float4>             primLo(m), primHi(m), boxLo(m), boxHi(m);
+    std::vector<unsigned long long> keys(M);
+    std::vector<int>                left(m), right(m), parentI(m), parentL(m);
+    std::vector<uint32_t>           first(m), last(m), visits(m, 0), triMeta((size_t)m * 2), counters(3, 0);
+    B.nodes.assign((size_t)m * 20 + 20, 0.f);
+    B.tris.assign((size_t)m * 12, 0.f);
+    int      cb[6] = {0x7fffffff, 0x7fffffff, 0x7fffffff, (int)0x80000000, (int)0x80000000, (int)0x80000000};
+    LbvhWork W{m, M, rec.data(), nullptr, primLo.data(), primHi.data(), keys.data(), left.data(), right.data(), parentI.data(), parentL.data(), first.data(),
+               last.data(), boxLo.data(), boxHi.data(), visits.data(), cb, B.nodes.data(), B.tris.data(), triMeta.data(), 0u, counters.data()};
+    for(uint32_t i = 0; i < m; i++) lbvhBounds(i, W);
+    for(uint32_t i = 0; i < M; i++) lbvhMorton(i, W);
+    for(uint32_t k = 2; k <= M; k <<= 1)
+      for(uint32_t j = k >> 1; j > 0; j >>= 1)
+        for(uint32_t t = 0; t < M; t++) bitonicStep(t, keys.data(), j, k);
+    for(uint32_t i = 0; i + 1 < m; i++) lbvhHierarchy(i, W);
+    for(uint32_t i = 0; i < m; i++) lbvhFit(i, W);
+    std::vector<int2> qa(m + 1), qb(m + 1);
+    qa[0] = make_int2(m >= 2 ? 0 : ~0, 0);
+    counters[0] = 1;
+    for(uint32_t count = 1; count;)
+    {
+      counters[2] = 0;
+      for(uint32_t q = 0; q < count; q++) lbvhEmit(q, W, qa.data(), qb.data());
+      count = counters[2];
+      std::swap(qa, qb);
+    }
+    B.numNodes = counters[0];
+    B.numTris = counters[1];
+  }
+  else
+    buildWideBvh(tris, gids, 0, B);
+  if(treeKind == 2)
+  {
+    // move every third triangle (by global id) in the tree's records, like k_refit_tris, then refit bottom-up by level
+    float lo[3] = {3e38f, 3e38f, 3e38f}, hi[3] = {-3e38f, -3e38f, -3e38f};
+    for(uint32_t i = 0; i < nT * 9; i++) lo[i % 3] = std::min(lo[i % 3], tv[i]), hi[i % 3] = std::max(hi[i % 3], tv[i]);
+    const float ext = std::max(hi[0] - lo[0], std::max(hi[1] - lo[1], hi[2] - lo[2]));
+    for(uint32_t s = 0; s < B.numTris; s++)
+    {
+      float*   T = &B.tris[(size_t)s * 12];
+      uint32_t gid; std::memcpy(&gid, &T[11], 4);
+      if(gid % 3u) continue;
+      T[0] += 0.05f * ext; T[1] = T[1] * 0.8f + 0.02f * ext; T[2] -= 0.03f * ext;
+      T[5] *= 0.8f; T[9] *= 0.8f;
+    }
+    std::vector<std::pair<uint32_t, uint32_t>> levels;
+    for(uint32_t first = 0, count = 1; count;)
+    {
+      levels.push_back({first, count});
+      uint32_t next = 0;
+      for(uint32_t n = first; n < first + count; n++) next += (uint32_t)__builtin_popcount(__float_as_uint(B.nodes[(size_t)n * 20 + 3]) >> 24);
+      first += count; count = next;
+    }
+    std::vector<float4> nodeBox((size_t)B.numNodes * 2);
+    for(size_t l = levels.size(); l-- > 0;)
+      for(uint32_t i = 0; i < levels[l].second; i++)
+        refitNode(levels[l].first + i, B.nodes.data(), B.tris.data(), nodeBox.data());
+  }
+  // the brute force runs over the tree's own records, each triangle exactly once
+  {
+    std::vector<int> seen(nT, 0);
+    for(uint32_t s = 0; s < B.numTris; s++) seen[__float_as_uint(B.tris[(size_t)s * 12 + 11])]++;
+    if(B.numTris != nT || std::count(seen.begin(), seen.end(), 1) != (long)nT) { std::printf("tree does not hold every triangle once\n"); return 1; }
+  }
   BvhView view{reinterpret_cast<const float4*>(B.nodes.data()), reinterpret_cast<const float4*>(B.tris.data())};
   // synthetic micromaps
   const uint32_t        ommLevel = argc > 4 ? (uint32_t)std::atoi(argv[4]) : 0u;
@@ -115,13 +199,14 @@ int main(int argc, char** argv)
   {
     const float* R = &rv[(size_t)r * 8];
     const float3 org = f3(R[0], R[1], R[2]), dir = f3(R[4], R[5], R[6]);
-    const float  tmin = 0.0f, tmax = (r & 1) ? R[7] : 3.0f;  // half the rays as bounded segments
+    const float  tmin = ownSegment ? R[3] : 0.0f, tmax = (ownSegment || (r & 1)) ? R[7] : 3.0f;  // half the rays as bounded segments
     // brute force with the kernel's own triangle arithmetic
     bf.clear();
-    for(uint32_t i = 0; i < nT; i++)
+    for(uint32_t s = 0; s < B.numTris; s++)
     {
-      const float3 v0 = f3(tris[i].v0[0], tris[i].v0[1], tris[i].v0[2]), e1 = f3(tris[i].e1[0], tris[i].e1[1], tris[i].e1[2]),
-                   e2 = f3(tris[i].e2[0], tris[i].e2[1], tris[i].e2[2]);
+      const float*   T = &B.tris[(size_t)s * 12];
+      const uint32_t i = __float_as_uint(T[11]);
+      const float3   v0 = f3(T[0], T[1], T[2]), e1 = f3(T[4], T[5], T[6]), e2 = f3(T[8], T[9], T[10]);
       const float3 pvec = crossFma(dir, e2);
       const float  det = dotFma(e1, pvec);
       const float  inv = 1.0f / det;
@@ -132,6 +217,11 @@ int main(int argc, char** argv)
       const float  t = dotFma(e2, qvec) * inv;
       if((det != 0.0f) & (u >= 0.0f) & (u <= 1.0f) & (v >= 0.0f) & (u + v <= 1.0f) & (t > tmin) & (t < tmax))
       {
+        if(hitsOut)
+        {
+          const float rec[6] = {__uint_as_float(r), __uint_as_float(i), t, u, v, det};
+          std::fwrite(rec, 4, 6, hitsOut);
+        }
         const int kind = effective(i, u, v);
         if(kind != OMM_TRANSPARENT)
           bf.push_back(BF{t, i, kind});
@@ -209,6 +299,8 @@ int main(int argc, char** argv)
       }
     }
   }
+  if(hitsOut)
+    std::fclose(hitsOut);
   std::printf("hit rate %.3f, %.2f candidates per ray, deepest stack %d of %d | mismatches: nearest opaque %llu, shadow %llu, candidates %llu\n", (double)hits / nR,
               (double)listed / nR, maxSp, TravState::kStackSize, (unsigned long long)bad1, (unsigned long long)bad2, (unsigned long long)bad3);
   if(maxSp >= TravState::kStackSize)

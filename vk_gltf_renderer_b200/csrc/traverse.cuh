@@ -63,6 +63,21 @@ PT_D uint32_t signExtendS8x4(uint32_t x)
 // (mantissa ulp 2^-6), giving 131072 + b exactly, in one IMAD-pipe instruction.  The bias moves into the addend:
 // t = (131072 + b) * ad + (ao - 131072 * ad); the addend's rounding error is at most |ad| / 128, the test widens by |ad| / 64.
 constexpr float kByteBias = 131072.0f, kByteSlack = 0.015625f;
+// The node test is conservative w.r.t. the triangle test (Ize, "Robust BVH Ray Traversal", JCGT 2013, applied to both sides of the
+// comparison).  Let e = 2^-24 and D = sum_a |n0_a - org_a| + 256 s_a (s_a the node's quantum), an upper bound on the L1 distance from
+// the origin to any point of the node, so on |org - v0| of every triangle under it and on t |dir| of every hit in it.
+//  - slab side: of (n0 - org) * id, the fma with -131072 ad, the widening and the fma with the biased byte, each rounding adds at most
+//    e |id_a| D (the operands are bounded by |id_a| D) except the two biased ones (|ad| / 128 each, kByteSlack above); the rounded
+//    reciprocal id moves the slab by e |id_a| D; fmaxf / fminf against tLow and bound are exact.  Together < |id_a| (s_a / 64 + 8 e D).
+//  - triangle side: tvec = org - v0 is rounded by e |tvec| per component, and every dot / cross product of the Moeller-Trumbore chain
+//    errs by a few e times the product of its operands' norms.  An accepted (t, u, v) is therefore exact for an origin moved by
+//    < 6 e D and a t that is off by < 6 e D / (|dir| sin(phi) cos(theta)) (phi: angle between e1 and e2, theta: between dir and the
+//    normal).  Both are points within 6 e D / (sin(phi) cos(theta)) of the triangle, so of the child box.
+// Widening each slab by |id_a| (s_a / 64 + kWalkEps D) covers both: |id_a| >= 1 / |dir| and t |dir| <= D make the margin at least
+// kWalkEps t, so kWalkEps = 256 e admits every hit with sin(phi) cos(theta) >= 6 / (256 - 8), i.e. all but triangles seen within
+// ~1.4 degrees of edge-on and slivers under ~1.4 degrees.  tests/test_walk_precision.py measures the t error of every brute-force hit;
+// the walks equal the brute force on every ray whose hits err by less than 192 e D, and the rest are counted.
+constexpr float kWalkEps = 1.52587890625e-05f;  // 2^-16
 // byte J of x as an integer (SHF + LOP3 on the ALU pipe; doing these two extractions per child with IDP.4A as well puts 64
 // instead of 48 instructions per node on the IMAD pipe, which then becomes the longer one)
 template <int J>
@@ -156,10 +171,12 @@ struct TravState
     tris = bvh.tris;
     org = o;
     dir = d;
+    // a component below ooeps is clamped with the sign step() and dsign read from `d.x < 0.f`: -0 counts as positive, so its slab
+    // is not inverted (a copysignf clamp gave -0 a negative reciprocal, and such a ray missed every node it started inside of)
     const float ooeps = 1e-20f;
-    const float dx = fabsf(d.x) > ooeps ? d.x : copysignf(ooeps, d.x);
-    const float dy = fabsf(d.y) > ooeps ? d.y : copysignf(ooeps, d.y);
-    const float dz = fabsf(d.z) > ooeps ? d.z : copysignf(ooeps, d.z);
+    const float dx = fabsf(d.x) > ooeps ? d.x : (d.x < 0.f ? -ooeps : ooeps);
+    const float dy = fabsf(d.y) > ooeps ? d.y : (d.y < 0.f ? -ooeps : ooeps);
+    const float dz = fabsf(d.z) > ooeps ? d.z : (d.z < 0.f ? -ooeps : ooeps);
     idx = 1.0f / dx;
     idy = 1.0f / dy;
     idz = 1.0f / dz;
@@ -259,16 +276,21 @@ struct TravState
         const float4 n4 = __ldg(&nodes[nodeIndex * 5 + 4]);
 
         const uint32_t eImask = __float_as_uint(n0.w);
-        const float    adx = __uint_as_float(extractByte(eImask, 0) << 23) * idx;
-        const float    ady = __uint_as_float(extractByte(eImask, 1) << 23) * idy;
-        const float    adz = __uint_as_float(extractByte(eImask, 2) << 23) * idz;
-        // quantised plane bytes -> floats with the bias folded into the addend, conservative slack (see biasedByte)
-        const float aox = fmaf(-kByteBias, adx, (n0.x - org.x) * idx);
-        const float aoy = fmaf(-kByteBias, ady, (n0.y - org.y) * idy);
-        const float aoz = fmaf(-kByteBias, adz, (n0.z - org.z) * idz);
-        const float aoxN = fmaf(-kByteSlack, fabsf(adx), aox), aoxF = fmaf(kByteSlack, fabsf(adx), aox);
-        const float aoyN = fmaf(-kByteSlack, fabsf(ady), aoy), aoyF = fmaf(kByteSlack, fabsf(ady), aoy);
-        const float aozN = fmaf(-kByteSlack, fabsf(adz), aoz), aozF = fmaf(kByteSlack, fabsf(adz), aoz);
+        const float    sx = __uint_as_float(extractByte(eImask, 0) << 23), sy = __uint_as_float(extractByte(eImask, 1) << 23);
+        const float    sz = __uint_as_float(extractByte(eImask, 2) << 23);
+        const float    adx = sx * idx, ady = sy * idy, adz = sz * idz;
+        const float    ox = n0.x - org.x, oy = n0.y - org.y, oz = n0.z - org.z;
+        // quantised plane bytes -> floats with the bias folded into the addend (see biasedByte); each slab widened by
+        // |id_a| (s_a kByteSlack + kWalkEps D) (see kWalkEps)
+        const float aox = fmaf(-kByteBias, adx, ox * idx);
+        const float aoy = fmaf(-kByteBias, ady, oy * idy);
+        const float aoz = fmaf(-kByteBias, adz, oz * idz);
+        const float reach = fmaf(256.0f * kWalkEps, sx + sy + sz, kWalkEps * (fabsf(ox) + fabsf(oy) + fabsf(oz)));
+        const float wx = fabsf(idx) * fmaf(kByteSlack, sx, reach), wy = fabsf(idy) * fmaf(kByteSlack, sy, reach);
+        const float wz = fabsf(idz) * fmaf(kByteSlack, sz, reach);
+        const float aoxN = aox - wx, aoxF = aox + wx;
+        const float aoyN = aoy - wy, aoyF = aoy + wy;
+        const float aozN = aoz - wz, aozF = aoz + wz;
 
         // per-node axis map (bvh.cpp): bit k of the node's octant mask is the direction sign along the axis slot bit k follows
         const uint32_t n1x = __float_as_uint(n1.x);
@@ -304,8 +326,7 @@ struct TravState
     const float tmaxz = fmaf(biasedByte<J>(zmax), adz, aozF);                                                              \
     const float tn = fmaxf(fmaxf(tminx, tminy), fmaxf(tminz, tLow));                                                       \
     const float tf = fminf(fminf(tmaxx, tmaxy), fminf(tmaxz, bound));                                                      \
-    /* widen by a few ulp: keeps the box test conservative w.r.t. the triangle test */                                     \
-    const bool     in = tn <= tf * 1.000001f;                                                                              \
+    const bool     in = tn <= tf;                                                                                          \
     const uint32_t childBits = in ? extractByteJ<J>(childBits4) : 0u;                                                      \
     hitMask |= childBits << extractByteJ<J>(bitIndex4);                                                                    \
   }

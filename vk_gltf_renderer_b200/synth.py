@@ -725,13 +725,18 @@ def synth_hierarchy(seed=1234):
     return scn, np.asarray(parents, np.int32), mappings, inst, pose
 
 
-def triangle_soup(n, seed=1234, extent=1.0, size=0.15):
-    """n random triangles in a cube: stress input for traversal parity tests."""
-    rng = np.random.default_rng(seed)
-    c = (rng.random((n, 1, 3)) - 0.5) * 2 * extent
-    v = c + (rng.random((n, 3, 3)) - 0.5) * 2 * size
+def triangle_soup(n, seed=1234, extent=1.0, size=0.15, vertices=None, double_sided=0, material=None):
+    """n random triangles in a cube: stress input for traversal parity tests.  vertices: (n, 3, 3) triangles to use instead;
+    material: add_material arguments that replace the default ones (e.g. an alpha mode)."""
+    if vertices is None:
+        rng = np.random.default_rng(seed)
+        c = (rng.random((n, 1, 3)) - 0.5) * 2 * extent
+        v = c + (rng.random((n, 3, 3)) - 0.5) * 2 * size
+    else:
+        v = np.asarray(vertices, np.float32)
+        n = len(v)
     scn = Scene()
-    m = scn.add_material(pbrBaseColorFactor=[0.8, 0.8, 0.8, 1], pbrMetallicFactor=0.0, doubleSided=0)
+    m = scn.add_material(**dict(dict(pbrBaseColorFactor=[0.8, 0.8, 0.8, 1], pbrMetallicFactor=0.0, doubleSided=double_sided), **(material or {})))
     p = scn.add_primitive(v.reshape(-1, 3), np.arange(n * 3).reshape(-1, 3))
     scn.add_node(p, m)
     return scn
